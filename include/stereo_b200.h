@@ -160,6 +160,30 @@ int sb_conv2d_simt(const sb_conv_desc* d, sb_stream_t stream);
 int sb_conv2d_tc(const sb_conv_desc* d, sb_stream_t stream);
 int sb_conv2d_tc_supported(const sb_conv_desc* d);
 
+/* ------------------------------------------------- backward pass of the trunk + FPN (fp16 operands, fp32 accumulate) ----
+ * sb_conv2d_tc_dgrad -- data gradient of a conv (the input gradient torch.nn.Conv2d's autograd forms for the convs of
+ *   lib/model/stereo_rcnn/resnet.py:66-102 and stereo_rcnn.py:91-108,155-168) as the forward implicit GEMM: d->in is the
+ *   fp16 output gradient, d->wgt the weights packed [Cin][kh][kw][Cout] with the taps flipped and the frozen-BN scale
+ *   folded in, Cin / Cout swapped in the descriptor.  The epilogue adds d->residual (1x1 only), then keeps an element
+ *   only where mask16 (fp16, the output's element layout; NULL = no mask) is > 0: the ReLU of the saved forward tensor.
+ *   d->relu, d->up_src and d->out_mode must be 0; out_strides scatter into even positions for stride-2 convs.
+ * sb_conv_wgrad -- weight gradient (and optionally bias gradient) of a 1x1 or 3x3 (pad 1) stride-1 conv:
+ *   dw[Cout][Cin][k][k] = scale[co] / grad_scale * sum_p dy16[p][co] x16[p + tap][ci] (NHWC fp16 operands, N x H x W),
+ *   db[co] = sum_p dy32[p][co] / grad_scale.  Split over pixel ranges, partials reduced in a fixed order: bit-identical
+ *   run to run.  *nonfinite (device int, may be NULL) is set to 1 when a result is not finite (never cleared).
+ *   Cin, Cout multiples of 64; workspace of sb_conv_wgrad_workspace bytes.
+ * sb_fpn_grad_combine -- gradient of one FPN level: out = scale * dp + up^T(dt) + scatter2(scale * dp6) over NHWC fp32
+ *   [N,H,W,C]; up^T transposes the align_corners bilinear upsample of stereo_rcnn.py:91-108 from the fine [N,TH,TW,C] dt
+ *   (a gather, fixed order); dp6 [N,H6,W6,C] is the gradient of P6 = P5[::2, ::2] (stereo_rcnn.py:168).  dp, dt and dp6
+ *   may each be NULL; out (fp32) and/or out16 (fp16 twin) receive the result.                                      */
+int sb_conv2d_tc_dgrad(const sb_conv_desc* d, const void* mask16, sb_stream_t stream);
+size_t sb_conv_wgrad_workspace(int N, int H, int W, int Cin, int Cout, int k);
+int sb_conv_wgrad(const void* dy16, const void* x16, int N, int H, int W, int Cin, int Cout, int k,
+                  const float* scale, float inv_grad_scale, float* dw, const float* dy32, float* db, int* nonfinite,
+                  void* workspace, size_t workspace_bytes, sb_stream_t stream);
+int sb_fpn_grad_combine(const float* dp, const float* dt, int N, int H, int W, int TH, int TW, int C,
+                        const float* dp6, int H6, int W6, float scale, float* out, void* out16, sb_stream_t stream);
+
 /* Diagnostics (tools/conv_trace.py): per-CTA phase timestamps of every following sb_conv2d_tc launch, 16 x u64
  * per CTA and 304 CTA slots per launch, into a caller-owned device buffer of sb_conv_trace_bytes(max_launches)
  * bytes.  buf = NULL switches tracing off.  No counterpart in the reference. */

@@ -58,6 +58,9 @@ struct TcParams {
     // STEM variant: the A operand is gathered from the NCHW fp32 image [N,3,sH,sW] (7x7 / stride 2 / pad 3 patches)
     const float* stem_im;
     int sH, sW;
+    // MASK variant (dgrad of the backward pass): output element e is kept only where mask16[e] > 0 (the ReLU mask of
+    // a saved forward tensor with the output's layout), after the residual add
+    const __half* mask16;
 };
 
 __device__ __forceinline__ unsigned long long gtimer() {
@@ -71,11 +74,12 @@ constexpr size_t conv_smem(int block_n, int stages) {
     return (size_t)stages * (BLOCK_M * kRowBytes + block_n * kRowBytes) + 1024 + 2 * stages * 8;
 }
 
-template <int BLOCK_N, int kStages, bool HAS_RES, bool HAS_UP, bool IN16, bool STEM = false>
+template <int BLOCK_N, int kStages, bool HAS_RES, bool HAS_UP, bool IN16, bool STEM = false, bool MASK = false>
 __global__ void __launch_bounds__(STEM ? kStemThreads : kThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                const TcParams p) {
     static_assert(!STEM || (IN16 && !HAS_RES && !HAS_UP), "stem variant");
+    static_assert(!MASK || (IN16 && !HAS_UP && !STEM), "mask variant");
     constexpr uint32_t kABytes = BLOCK_M * kRowBytes, kBBytes = BLOCK_N * kRowBytes;
     constexpr int BLOCK_K = IN16 ? 64 : 32;     // elements per K-step
     constexpr uint32_t kStageBytes = kABytes + kBBytes;
@@ -344,6 +348,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                         x0 += ly0 * (lx0 * a.x + lx1 * bq.x) + ly1 * (lx0 * g.x + lx1 * hh.x);
                         x1 += ly0 * (lx0 * a.y + lx1 * bq.y) + ly1 * (lx0 * g.y + lx1 * hh.y);
                     }
+                    if (MASK) {
+                        const __half2 mk = *reinterpret_cast<const __half2*>(p.mask16 + ooff[h] + c);
+                        if (!(__low2float(mk) > 0.f)) x0 = 0.f;
+                        if (!(__high2float(mk) > 0.f)) x1 = 0.f;
+                    }
                     if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
                     if (out_mode == 1) { x0 = sb_round_tf32(x0); x1 = sb_round_tf32(x1); }
                     else if (out_mode == 2) { x0 = sb_bias_tf32(x0); x1 = sb_bias_tf32(x1); }
@@ -406,11 +415,11 @@ int pick_block_n(int cout, long long m_tiles, int num_sms) {
     return c256 <= c128 ? 256 : 128;
 }
 
-template <int BN, int ST, bool RES, bool UP, bool IN16, bool STEM = false>
+template <int BN, int ST, bool RES, bool UP, bool IN16, bool STEM = false, bool MASK = false>
 int launch_t(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& p, cudaStream_t st) {
     constexpr size_t smem = conv_smem(BN, ST);
     static_assert(smem <= 227 * 1024, "smem budget");
-    auto kern = conv_tc_kernel<BN, ST, RES, UP, IN16, STEM>;
+    auto kern = conv_tc_kernel<BN, ST, RES, UP, IN16, STEM, MASK>;
     static bool attr_done[kSbMaxDevices] = {false};
     bool& attr = attr_done[sb_cur_device()];
     if (!attr) {
@@ -443,6 +452,9 @@ int launch_t(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& p, cu
 template <int BN, int ST>
 int launch(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& p, cudaStream_t st) {
     const bool res = p.d.residual != nullptr, up = p.d.up_src != nullptr;   // never both (supported())
+    if (p.mask16)       // dgrad: fp16 operands, never an upsample source (sb_conv2d_tc_dgrad)
+        return res ? launch_t<BN, ST, true, false, true, false, true>(ma, mb, p, st)
+                   : launch_t<BN, ST, false, false, true, false, true>(ma, mb, p, st);
     if (p.d.in_dtype == 1) {
         if (up) return launch_t<BN, ST, false, true, true>(ma, mb, p, st);
         return res ? launch_t<BN, ST, true, false, true>(ma, mb, p, st) : launch_t<BN, ST, false, false, true>(ma, mb, p, st);
@@ -503,10 +515,12 @@ extern "C" int sb_conv_trace_info(int id, int* out12) {
 }
 extern "C" int sb_conv_trace_count(void) { return g_trace_n; }
 
-extern "C" int sb_conv2d_tc(const sb_conv_desc* d, sb_stream_t stream) {
+namespace {
+int conv2d_tc(const sb_conv_desc* d, const __half* mask16, sb_stream_t stream) {
     if (!sb_conv2d_tc_supported(d)) return SB_EINVAL;
     TcParams p;
     p.d = *d;
+    p.mask16 = mask16;
     // default: release the dependent launch once this CTA's last operand loads are issued -- an early release lets
     // the next kernel's CTAs sit in griddepcontrol.wait on SMs the other stream's chain could be using
     static const bool pdl_late = getenv("SB_PDL_LATE") == nullptr || atoi(getenv("SB_PDL_LATE")) != 0;
@@ -569,6 +583,19 @@ extern "C" int sb_conv2d_tc(const sb_conv_desc* d, sb_stream_t stream) {
         default: return launch<128, 6>(ma, mb, p, st);
     }
 }
+}  // namespace
+
+extern "C" int sb_conv2d_tc(const sb_conv_desc* d, sb_stream_t stream) { return conv2d_tc(d, nullptr, stream); }
+
+// Data gradient of a convolution as the forward implicit GEMM on transposed weights (the caller packs them
+// [Cin][kh][kw][Cout], taps flipped, frozen-BN scale folded in), with the ReLU mask of a saved tensor applied after
+// the optional residual add.  mask16 has the output's element layout (out strides and channel offset).
+extern "C" int sb_conv2d_tc_dgrad(const sb_conv_desc* d, const void* mask16, sb_stream_t stream) {
+    if (!d || d->in_dtype != 1 || d->up_src || d->relu || d->out_mode != 0) return SB_EINVAL;
+    if (reinterpret_cast<uintptr_t>(mask16) & 3) return SB_EINVAL;
+    if (!mask16) return conv2d_tc(d, nullptr, stream);
+    return conv2d_tc(d, reinterpret_cast<const __half*>(mask16), stream);
+}
 
 // The stem (resnet.py:111-112: Conv2d(3, 64, 7, stride 2, pad 3) + frozen BN + ReLU) as an implicit GEMM on the tensor
 // cores, patches gathered inside the kernel (conv_tc_kernel<.., STEM>): image NCHW fp32 [N,3,H,W], weights fp16
@@ -595,6 +622,7 @@ extern "C" int sb_stem_conv_tc(const float* im_nchw, int N, int H, int W, const 
     static const bool pdl_late = getenv("SB_PDL_LATE") == nullptr || atoi(getenv("SB_PDL_LATE")) != 0;
     p.pdl_late = pdl_late ? 1 : 0;
     p.stem_im = im_nchw; p.sH = H; p.sW = W;
+    p.mask16 = nullptr;
     CUtensorMap mb;
     {
         cuuint64_t dims[2] = {192, 64};

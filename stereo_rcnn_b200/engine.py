@@ -21,6 +21,47 @@ def _pack_conv(w):
     return w.permute(0, 2, 3, 1).contiguous()
 
 
+def trainable_trunk_fpn_params(fixed_blocks=1):
+    """[(name, shape)] of the trunk + FPN parameters that receive a gradient (resnet.py:289-309 of the reference):
+    RCNN_layer0 and every BatchNorm are frozen, cfg.RESNET.FIXED_BLOCKS = k also freezes RCNN_layer1..k, the FPN convs
+    (top, lateral and smooth layers, weights and biases) always train."""
+    assert 0 <= fixed_blocks < 4
+    out = []
+    inplanes = 64
+    for li, nb in enumerate(LAYERS):
+        planes = PLANES[li]
+        for bi in range(nb):
+            p = "RCNN_layer%d.0.%d" % (li + 1, bi)
+            cin = inplanes if bi == 0 else planes * 4
+            if li + 1 > fixed_blocks:
+                out += [(p + ".conv1.weight", (planes, cin, 1, 1)), (p + ".conv2.weight", (planes, planes, 3, 3)),
+                        (p + ".conv3.weight", (planes * 4, planes, 1, 1))]
+                if bi == 0:
+                    out.append((p + ".downsample.0.weight", (planes * 4, cin, 1, 1)))
+        inplanes = planes * 4
+    for k, cin, ks in (("RCNN_toplayer", 2048, 1), ("RCNN_smooth1", 256, 3), ("RCNN_smooth2", 256, 3),
+                       ("RCNN_smooth3", 256, 3), ("RCNN_latlayer1", 1024, 1), ("RCNN_latlayer2", 512, 1),
+                       ("RCNN_latlayer3", 256, 1)):
+        out += [(k + ".weight", (256, cin, ks, ks)), (k + ".bias", (256,))]
+    return out
+
+
+# which lateral conv reads the input of RCNN_layer<li+1> (li = 1..3): c2 -> latlayer3, c3 -> latlayer2, c4 -> latlayer1
+_LATERAL_OF_INPUT = {1: ("RCNN_latlayer3", "dt2"), 2: ("RCNN_latlayer2", "dt3"), 3: ("RCNN_latlayer1", "dt4")}
+
+
+class _DgradConv(object):
+    """conv weights for the data gradient: [Cin][kh][kw][Cout] fp16, taps flipped, frozen-BN scale folded in"""
+    __slots__ = ("w16", "Cin", "Cout", "kh", "kw", "pad")
+
+    def __init__(self, w, scale, pad, device):
+        co, ci, self.kh, self.kw = w.shape
+        if scale is not None:
+            w = w * scale.view(-1, 1, 1, 1)
+        self.w16 = w.flip(2, 3).permute(1, 2, 3, 0).contiguous().to(torch.float16).to(device)
+        self.Cin, self.Cout, self.pad = co, ci, pad
+
+
 class PackedConv(object):
     __slots__ = ("w", "w16", "scale", "shift", "Cin", "Cout", "kh", "kw", "pad")
 
@@ -76,6 +117,11 @@ class StereoRCNNEngine(object):
         sd = {k: v.detach().to("cpu", torch.float32) for k, v in state_dict.items()
               if not k.endswith("num_batches_tracked")}
         self.p = {}
+        # exact host weights and BN scales of the trunk + FPN convs, for the backward's transposed weights (packed on
+        # the device only when a backward is first requested)
+        self._bwd_src = {}
+        self._bwd = None
+        self._found_inf = None
 
         def bn_fold(k):
             s = sd[k + ".weight"] / torch.sqrt(sd[k + ".running_var"] + EPS)
@@ -84,9 +130,13 @@ class StereoRCNNEngine(object):
         def conv_bn(ck, bk, pad):
             s, b = bn_fold(bk)
             self.p[ck] = PackedConv(sd[ck + ".weight"], s, b, pad)
+            if ck.startswith("RCNN_layer"):
+                self._bwd_src[ck] = (sd[ck + ".weight"], s, pad)
 
         def conv_bias(ck, pad):
             self.p[ck] = PackedConv(sd[ck + ".weight"], None, sd[ck + ".bias"].contiguous(), pad)
+            if not ck.startswith("RCNN_rpn"):
+                self._bwd_src[ck] = (sd[ck + ".weight"], None, pad)
 
         # stem: [64,3,7,7] -> [64][7][7][3]
         s, b = bn_fold("RCNN_layer0.1")
@@ -186,22 +236,30 @@ class StereoRCNNEngine(object):
         return self._conv(o, self.p[prefix + ".conv3"], relu=True, residual=res, tag=prefix + ".conv3",
                           out_mode=ops.BIASED, res_biased=not has_ds)
 
-    def _bottleneck16(self, x32, x16, prefix, stride, has_ds, out=None):
+    def _bottleneck16(self, x32, x16, prefix, stride, has_ds, out=None, saved=None):
         """fp16-operand variant: convs read fp16 twins, the residual stream itself stays exact fp32.
-        out = (fp32 view, fp16 view) to write the block output into (slices of a batched tensor)"""
+        out = (fp32 view, fp16 view) to write the block output into (slices of a batched tensor).
+        saved: dict that receives the conv inputs the backward needs (fp16 twins, all ReLU'd)"""
         xin = ops.subsample2(x16) if stride == 2 else x16
-        o = self._conv(xin, self.p[prefix + ".conv1"], relu=True, tag=prefix + ".conv1", f32=False, f16=True)
-        o = self._conv(o, self.p[prefix + ".conv2"], relu=True, tag=prefix + ".conv2", f32=False, f16=True)
+        o1 = self._conv(xin, self.p[prefix + ".conv1"], relu=True, tag=prefix + ".conv1", f32=False, f16=True)
+        o = self._conv(o1, self.p[prefix + ".conv2"], relu=True, tag=prefix + ".conv2", f32=False, f16=True)
         res = self._conv(xin, self.p[prefix + ".downsample.0"], tag=prefix + ".ds") if has_ds else x32
+        if saved is not None:
+            saved[prefix] = dict(xin=xin, o1=o1, o2=o)
         if out is not None:
             return self._conv(o, self.p[prefix + ".conv3"], relu=True, residual=res, tag=prefix + ".conv3",
                               out=out[0], out16=out[1])
         return self._conv(o, self.p[prefix + ".conv3"], relu=True, residual=res, tag=prefix + ".conv3", f16=True)
 
-    def trunk_fpn(self, im_nchw):
-        """images [N,3,H,W] NCHW -> dict of NHWC C2..C5, P2..P6 (stereo_rcnn.py:155-168)"""
+    def trunk_fpn(self, im_nchw, save_for_backward=False):
+        """images [N,3,H,W] NCHW -> dict of NHWC C2..C5, P2..P6 (stereo_rcnn.py:155-168).
+        save_for_backward=True (fp16-operand engines) returns (feats, saved): `saved` keeps the conv inputs (the fp16
+        twins the forward consumed, all ReLU'd) that trunk_fpn_backward needs.  The left and the right image then run
+        layers 3-4 as one batched chain; every value computed is the same."""
         if self.half:
-            return self._trunk_fpn16(im_nchw)
+            return self._trunk_fpn16(im_nchw, save_for_backward)
+        if save_for_backward:
+            raise ValueError("the backward pass runs on fp16 conv operands: build the engine with precision='fp16'")
         if self.exact:
             c0 = ops.stem_conv(im_nchw, *self.stem, out_mode=ops.EXACT)
         else:       # patch matrix (pixels rounded to TF32) + tensor-core GEMM
@@ -225,7 +283,7 @@ class StereoRCNNEngine(object):
         feats.update(p2=p2, p3=p3, p4=p4, p5=p5, p6=p6)
         return feats
 
-    def _trunk_fpn16(self, im_nchw):
+    def _trunk_fpn16(self, im_nchw, save_for_backward=False):
         """fp16-operand trunk: every conv input is an fp16 tensor (half the HBM bytes, f16 = 2x the TF32
         MMA rate, same 11-bit significand); fp32 copies exist only where a non-conv consumer needs them
         (residual adds, FPN upsample source, RoIAlign, the user-visible P levels)."""
@@ -237,11 +295,12 @@ class StereoRCNNEngine(object):
             c0 = self._conv(ops.stem_im2col16(im_nchw), self.p["stem_gemm16"], relu=True, tag="stem", f32=False, f16=True)
         c1 = ops.maxpool3x3s2_ceil(c0)
         feats = {"c1": c1.float() if self.keep32 else None, "c1_16": c1}
+        saved = {} if save_for_backward else None
         x32, x16 = None, c1
         for li in (0, 1):                           # layers 1-2: left and right batched (hundreds of tiles)
             for bi in range(LAYERS[li]):
                 x32, x16 = self._bottleneck16(x32, x16, "RCNN_layer%d.0.%d" % (li + 1, bi),
-                                              STRIDES[li] if bi == 0 else 1, bi == 0)
+                                              STRIDES[li] if bi == 0 else 1, bi == 0, saved=saved)
             feats["c%d" % (li + 2)], feats["c%d_16" % (li + 2)] = x32, x16
         # layers 3-4 have 38 / 10 row tiles per image: far too few to fill 132 SMs, and every launch is latency
         # bound (prologue + load latency + main loop + epilogue back to back).  The left and the right image are
@@ -268,8 +327,8 @@ class StereoRCNNEngine(object):
                     last = bi == LAYERS[li] - 1
                     y32, y16 = self._bottleneck16(y32, y16, "RCNN_layer%d.0.%d" % (li + 1, bi),
                                                   STRIDES[li] if bi == 0 else 1, bi == 0,
-                                                  out=(dst[0][sl], dst[1][sl]) if last else None)
-        if self.side is not None and self.lr_streams:
+                                                  out=(dst[0][sl], dst[1][sl]) if last else None, saved=saved)
+        if self.side is not None and self.lr_streams and saved is None:
             main = torch.cuda.current_stream()
             self.side.wait_stream(main)
             self.max_ctas = self.chain_ctas      # each chain keeps to half of the SMs so that both really co-run
@@ -282,15 +341,117 @@ class StereoRCNNEngine(object):
             chain(slice(0, N))
         feats.update(c4=c4[0], c4_16=c4[1], c5=c5[0], c5_16=c5[1])
         p5, p5h = self._conv(feats["c5_16"], self.p["RCNN_toplayer"], tag="toplayer", f16=True)
-        t = self._conv(feats["c4_16"], self.p["RCNN_latlayer1"], up_src=p5, tag="lat1", f32=False, f16=True)
-        p4, p4h = self._conv(t, self.p["RCNN_smooth1"], tag="smooth1", f16=True)
-        t = self._conv(feats["c3_16"], self.p["RCNN_latlayer2"], up_src=p4, tag="lat2", f32=False, f16=True)
-        p3, p3h = self._conv(t, self.p["RCNN_smooth2"], tag="smooth2", f16=True)
-        t = self._conv(feats["c2_16"], self.p["RCNN_latlayer3"], up_src=p3, tag="lat3", f32=False, f16=True)
-        p2, p2h = self._conv(t, self.p["RCNN_smooth3"], tag="smooth3", f16=True)
+        t4 = self._conv(feats["c4_16"], self.p["RCNN_latlayer1"], up_src=p5, tag="lat1", f32=False, f16=True)
+        p4, p4h = self._conv(t4, self.p["RCNN_smooth1"], tag="smooth1", f16=True)
+        t3 = self._conv(feats["c3_16"], self.p["RCNN_latlayer2"], up_src=p4, tag="lat2", f32=False, f16=True)
+        p3, p3h = self._conv(t3, self.p["RCNN_smooth2"], tag="smooth2", f16=True)
+        t2 = self._conv(feats["c2_16"], self.p["RCNN_latlayer3"], up_src=p3, tag="lat3", f32=False, f16=True)
+        p2, p2h = self._conv(t2, self.p["RCNN_smooth3"], tag="smooth3", f16=True)
         feats.update(p2=p2, p3=p3, p4=p4, p5=p5, p6=ops.subsample2(p5), p2_16=p2h, p3_16=p3h, p4_16=p4h,
                      p5_16=p5h, p6_16=ops.subsample2(p5h))
+        if saved is not None:
+            saved.update(c2=feats["c2_16"], c3=feats["c3_16"], c4=feats["c4_16"], c5=feats["c5_16"], t2=t2, t3=t3,
+                         t4=t4)
+            return feats, saved
         return feats
+
+    # ------------------------------------------------------------------ backward of the trunk + FPN
+    def _pack_backward(self):
+        if self._bwd is None:
+            self._bwd = {k: _DgradConv(w, s, pad, self.device) for k, (w, s, pad) in self._bwd_src.items()}
+            self._found_inf = torch.zeros(4, dtype=torch.int32, device=self.device)   # [0]; sb_fill writes 4-word units
+        return self._bwd
+
+    @property
+    def found_inf(self):
+        """int32 [1] device flag: 1 when the last trunk_fpn_backward produced a non-finite gradient (cleared at the
+        start of every backward, never read on the host here -- torch.cuda.amp.GradScaler's found_inf)"""
+        self._pack_backward()
+        return self._found_inf[:1]
+
+    def _dgrad(self, dy16, key, out=None, out16=None, residual=None, mask=None, out_strides=None, f32=True,
+               f16=True):
+        """input gradient of conv `key` from the fp16 output gradient dy16 (stride 1; stride-2 callers scatter
+        through out / out_strides)"""
+        pc = self._bwd[key]
+        N, H, W = dy16.shape[:3]
+        if out is None and f32:
+            out = torch.empty(N, H, W, pc.Cout, dtype=torch.float32, device=dy16.device)
+        if out16 is None and f16:
+            out16 = torch.empty(N, H, W, pc.Cout, dtype=torch.float16, device=dy16.device)
+        d = ops.conv_desc(dy16, pc.w16, out, pc.Cin, pc.Cout, pc.kh, pc.kw, 1, pc.pad, H, W, residual=residual,
+                          out16=out16, out_strides=out_strides)
+        ops.conv2d_dgrad(d, mask)
+        return out, out16
+
+    def _wgrad(self, grads, key, dy16, x16, gs, dy32=None):
+        pc = self.p[key]
+        ops.conv_wgrad(dy16, x16, pc.kh, grads[key + ".weight"], scale=pc.scale if dy32 is None else None,
+                       grad_scale=gs, dy32=dy32, db=grads[key + ".bias"] if dy32 is not None else None,
+                       nonfinite=self._found_inf)
+
+    def trunk_fpn_backward(self, saved, d_feats, fixed_blocks=1, grads=None, grad_scale=1.0):
+        """Backward of trunk_fpn (ResNet-101 layers 1-4 + FPN, frozen BN) for the gradients d_feats["p2".."p6"] (fp32
+        NHWC, the shapes trunk_fpn returns; left and right images batched, so every weight gradient sums over both).
+        Returns {state_dict name: fp32 gradient} of exactly trainable_trunk_fpn_params(fixed_blocks), in the
+        reference's layout; tensors given in `grads` (e.g. GradientBuckets views) are written in place.
+        grad_scale (a power of two) multiplies dP before the fp16 chain and is divided out of the results exactly;
+        found_inf is set when a result is not finite.  No host synchronisation: graph-capturable."""
+        self._pack_backward()
+        dev = self.device
+        gs = float(grad_scale)
+        out = {}
+        for name, shape in trainable_trunk_fpn_params(fixed_blocks):
+            g = grads.get(name) if grads is not None else None
+            if g is None:
+                g = torch.empty(shape, dtype=torch.float32, device=dev)
+            assert tuple(g.shape) == tuple(shape) and g.dtype == torch.float32 and g.is_contiguous(), name
+            out[name] = g
+        ops.fill_(self._found_inf, 0.0)
+        dp = {k: ops._f32c(d_feats[k]) for k in ("p2", "p3", "p4", "p5", "p6")}
+        # ---- FPN (stereo_rcnn.py:155-168): P2 <- smooth3(lat3(c2) + up(P3)) ... P5 = toplayer(c5), P6 = P5[::2, ::2]
+        g32, g16 = ops.fpn_grad_combine(dp["p2"], scale=gs)
+        dt = {}
+        for lvl, smooth, lat, tk, ck in ((2, "RCNN_smooth3", "RCNN_latlayer3", "t2", "c2"),
+                                         (3, "RCNN_smooth2", "RCNN_latlayer2", "t3", "c3"),
+                                         (4, "RCNN_smooth1", "RCNN_latlayer1", "t4", "c4")):
+            self._wgrad(out, smooth, g16, saved[tk], gs, dy32=g32)
+            t32, t16 = self._dgrad(g16, smooth)
+            self._wgrad(out, lat, t16, saved[ck], gs, dy32=t32)
+            dt["dt%d" % lvl] = t16
+            g32, g16 = ops.fpn_grad_combine(dp["p%d" % (lvl + 1)], dt=t32, dp6=dp["p6"] if lvl == 4 else None,
+                                            scale=gs)
+        self._wgrad(out, "RCNN_toplayer", g16, saved["c5"], gs, dy32=g32)
+        # gradient at the pre-ReLU sum of layer 4's last block: toplayer's input gradient masked by c5 > 0
+        g32, g16 = self._dgrad(g16, "RCNN_toplayer", mask=saved["c5"])
+        # ---- trunk (resnet.py:66-102, stride on conv1 and the downsample), top layer first
+        for li in range(3, fixed_blocks - 1, -1):
+            for bi in range(LAYERS[li] - 1, -1, -1):
+                p = "RCNN_layer%d.0.%d" % (li + 1, bi)
+                r = saved[p]
+                self._wgrad(out, p + ".conv3", g16, r["o2"], gs)
+                _, g2 = self._dgrad(g16, p + ".conv3", mask=r["o2"], f32=False)
+                self._wgrad(out, p + ".conv2", g2, r["o1"], gs)
+                _, g1 = self._dgrad(g2, p + ".conv2", mask=r["o1"], f32=False)
+                self._wgrad(out, p + ".conv1", g1, r["xin"], gs)
+                if bi > 0:      # identity shortcut: input grad = conv1's + the block's own, masked by the input's ReLU
+                    g32, g16 = self._dgrad(g1, p + ".conv1", residual=g32, mask=r["xin"])
+                    continue
+                self._wgrad(out, p + ".downsample.0", g16, r["xin"], gs)
+                if li <= fixed_blocks:      # the layer below is frozen: no gradient into its output
+                    break
+                # stride-2 first block: conv1 + downsample input gradients at the strided pixels, scattered into the
+                # even positions of the input (subsample2's backward); the lateral conv reading the same tensor
+                # adds its part and the input's ReLU mask applies
+                ds32, _ = self._dgrad(g16, p + ".downsample.0", f16=False)
+                lat, dtk = _LATERAL_OF_INPUT[li]
+                xf = saved["c%d" % (li + 1)]
+                N, Hf, Wf, C = xf.shape
+                scat = ops.fill_(torch.empty(N, Hf, Wf, C, dtype=torch.float32, device=dev), 0.0)
+                self._dgrad(g1, p + ".conv1", out=scat, residual=ds32, f16=False,
+                            out_strides=(Hf * Wf * C, 2 * Wf * C, 2 * C))
+                g32, g16 = self._dgrad(dt[dtk], lat, residual=scat, mask=xf)
+        return out
 
     def rpn(self, feats, B):
         """stereo_rpn.py:73-95 -> cls_prob [B,A,2], bbox_pred [B,A,6], level shapes"""

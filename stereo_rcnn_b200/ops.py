@@ -361,6 +361,62 @@ def conv2d(desc, impl="auto"):
     return impl
 
 
+def conv2d_dgrad(desc, mask16=None):
+    """data gradient through the tensor-core conv (desc built on transposed weights, see sb_conv2d_tc_dgrad);
+    mask16: fp16 tensor with the output's layout whose ReLU mask (> 0) is applied after the residual add"""
+    L = _l.load()
+    check(L.sb_conv2d_tc_dgrad(ctypes.byref(desc), ptr(mask16), stream_ptr()), "sb_conv2d_tc_dgrad")
+
+
+def conv_wgrad(dy16, x16, k, dw, scale=None, grad_scale=1.0, dy32=None, db=None, nonfinite=None):
+    """weight (and bias) gradient of a k x k (pad k // 2) stride-1 conv: dy16 [N,H,W,Cout], x16 [N,H,W,Cin] fp16 NHWC
+    -> dw [Cout,Cin,k,k] = scale[co] / grad_scale * sum dy x, db [Cout] = sum dy32 / grad_scale (fp32, written in
+    place); nonfinite: int32 [1] device flag set to 1 on a non-finite result"""
+    L = _l.load()
+    N, H, W, Cout = dy16.shape
+    Cin = x16.shape[3]
+    assert dy16.dtype == torch.float16 and x16.dtype == torch.float16 and tuple(x16.shape[:3]) == (N, H, W)
+    assert tuple(dw.shape) == (Cout, Cin, k, k) and dw.dtype == torch.float32
+    nb = L.sb_conv_wgrad_workspace(N, H, W, Cin, Cout, k)
+    ws = workspace(nb, dy16.device, "wgrad")
+    check(L.sb_conv_wgrad(ptr(dy16), ptr(x16), N, H, W, Cin, Cout, k, ptr(scale), float(1.0 / grad_scale), ptr(dw),
+                          ptr(dy32), ptr(db), ptr(nonfinite), ptr(ws), nb, stream_ptr()), "sb_conv_wgrad")
+    return dw, db
+
+
+def fpn_grad_combine(dp=None, dt=None, dp6=None, scale=1.0, shape=None, out=None, out16=None, f32=True, f16=True):
+    """gradient of one FPN level (NHWC fp32): scale * dp + up^T(dt) + scatter2(scale * dp6), where up^T is the
+    transpose of the align_corners bilinear upsample from this level to dt's size and scatter2 the backward of
+    P6 = P5[::2, ::2].  shape = (N, H, W, C) when dp is None.  Returns (fp32, fp16) as requested."""
+    L = _l.load()
+    N, H, W, C = dp.shape if dp is not None else shape
+    dev = (dp if dp is not None else dt).device
+    if out is None and f32:
+        out = torch.empty(N, H, W, C, dtype=torch.float32, device=dev)
+    if out16 is None and f16:
+        out16 = torch.empty(N, H, W, C, dtype=torch.float16, device=dev)
+    TH, TW = (dt.shape[1], dt.shape[2]) if dt is not None else (0, 0)
+    H6, W6 = (dp6.shape[1], dp6.shape[2]) if dp6 is not None else (0, 0)
+    for t in (dp, dt, dp6):
+        assert t is None or (t.dtype == torch.float32 and t.shape[0] == N and t.shape[3] == C)
+    check(L.sb_fpn_grad_combine(ptr(dp), ptr(dt), N, H, W, TH, TW, C, ptr(dp6), H6, W6, float(scale), ptr(out),
+                                ptr(out16), stream_ptr()), "sb_fpn_grad_combine")
+    return out, out16
+
+
+def upsample_transpose(dt, H, W):
+    """transpose of the align_corners bilinear upsample [N,H,W,C] -> [N,TH,TW,C] applied to dt (NHWC fp32)"""
+    return fpn_grad_combine(dt=dt, shape=(dt.shape[0], H, W, dt.shape[3]), f16=False)[0]
+
+
+def fill_(t, v=0.0):
+    """t[...] = v for a contiguous 4-byte-element CUDA tensor (sb_fill)"""
+    L = _l.load()
+    assert t.element_size() == 4
+    check(L.sb_fill(ptr(t), t.numel(), float(v), stream_ptr()), "sb_fill")
+    return t
+
+
 def stem_conv(im_nchw, wgt, scale, shift, out_mode=0):
     L = _l.load()
     N, _, H, W = im_nchw.shape
