@@ -156,7 +156,9 @@ typedef struct {
 } sb_conv_desc;
 
 int sb_conv2d_simt(const sb_conv_desc* d, sb_stream_t stream);
-/* tensor-core path: requires Cin % 32 == 0 (K tile = one 128-byte swizzle row), stride 1. */
+/* tensor-core path: requires Cin % 32 == 0 (K tile = one 128-byte swizzle row), stride 1.  With fp16 operands and a
+ * residual, the outputs leave by TMA: output pixels must be contiguous rows (h / n strides = Wo / Ho*Wo pixel
+ * strides), and with a twin out_w_stride and out_coff % 8 == 0 and out16 16-byte aligned. */
 int sb_conv2d_tc(const sb_conv_desc* d, sb_stream_t stream);
 int sb_conv2d_tc_supported(const sb_conv_desc* d);
 

@@ -23,13 +23,25 @@
 //     the next tile while the consumers finish the epilogue of the current one.
 //   * fused epilogue straight out of the accumulator registers: folded frozen-BN scale/shift or bias, residual add,
 //     FPN bilinear (align_corners) upsample-add, ReLU, the TF32 store modes, fp32 and/or fp16 ("twin") stores with
-//     arbitrary n/h/w strides and channel offset (RPN L|R concat, deconv scatter).
+//     arbitrary n/h/w strides and channel offset (RPN L|R concat, deconv scatter).  All loads of a column step (both
+//     rows: residual, the four upsample taps, scale / shift) are issued before its first store.
+//   * residual epilogue by TMA (fp16 operands, forward: conv3 of every bottleneck, HBM-bound): per consumer warpgroup
+//     a shared-memory buffer of its 64 rows -- BLOCK_N / 32 fp32 boxes of 64 x 32 (residual in, result out in place)
+//     and ceil(BLOCK_N / 64) fp16 boxes of 64 x 64 (the twin), 128-byte swizzled -- on its own full / empty mbarrier
+//     pair.  The producer requests tile t's residual boxes right after the first min(K-steps, stages) operand loads of
+//     tile t, so they land during tile t's main loop.  The consumers add the accumulators in place, write the twin,
+//     fence the async proxy and sync the warpgroup (named barrier); one thread issues the bulk tensor stores, waits
+//     until they have read the buffer (cp.async.bulk.wait_group.read) and releases it, and the warpgroup goes on to
+//     the next tile's MMAs while the stores drain to HBM.  Shared memory of a 128-wide residual tile: 4 operand
+//     stages of 32 KB + 2 warpgroups x (32 KB fp32 + 16 KB fp16) = 96 KB of epilogue buffers (64-wide: 7 x 24 KB +
+//     48 KB; 32-wide: 9 x 20 KB + 32 KB).  The TF32 mode and the data-gradient variants keep the register epilogue.
 //   * programmatic dependent launch: the prologue (barrier init, descriptor prefetch) overlaps the previous
 //     kernel's tail; dependents are released after the CTA's last operand loads are issued.
 //   * optional per-CTA phase trace (sb_conv_trace) for tools/conv_trace.py.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <stdlib.h>
+#include <string.h>
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -70,23 +82,39 @@ __device__ __forceinline__ unsigned long long gtimer() {
 }
 constexpr int kTraceWords = 16, kTraceCtas = 304;
 
-constexpr size_t conv_smem(int block_n, int stages) {
-    return (size_t)stages * (BLOCK_M * kRowBytes + block_n * kRowBytes) + 1024 + 2 * stages * 8;
+// TMA residual epilogue (fp16-operand forward with a residual): per consumer warpgroup, its 64 rows of the tile as
+// BLOCK_N / 32 fp32 boxes [64 rows][32 columns] (residual in, fp32 result out, in place) and ceil(BLOCK_N / 64) fp16
+// boxes [64 rows][64 columns] (the twin); every box is 64 x 128 bytes, 128-byte swizzled.
+constexpr uint32_t kEpiBox = 64 * 128;
+constexpr bool tma_epilogue(bool has_res, bool in16, bool mask) { return has_res && in16 && !mask; }
+constexpr uint32_t epi_res_bytes(int block_n) { return (uint32_t)(block_n / 32) * kEpiBox; }
+constexpr uint32_t epi_twin_bytes(int block_n) { return (uint32_t)((block_n + 63) / 64) * kEpiBox; }
+constexpr uint32_t epi_bytes(int block_n) { return 2 * (epi_res_bytes(block_n) + epi_twin_bytes(block_n)); }
+
+constexpr size_t conv_smem(int block_n, int stages, uint32_t epi) {
+    return (size_t)stages * (BLOCK_M * kRowBytes + block_n * kRowBytes) + epi + 1024 + (2 * stages + 4) * 8;
 }
 
 template <int BLOCK_N, int kStages, bool HAS_RES, bool HAS_UP, bool IN16, bool STEM = false, bool MASK = false>
 __global__ void __launch_bounds__(STEM ? kStemThreads : kThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-               const TcParams p) {
+               const __grid_constant__ CUtensorMap map_r, const __grid_constant__ CUtensorMap map_o,
+               const __grid_constant__ CUtensorMap map_o16, const TcParams p) {
     static_assert(!STEM || (IN16 && !HAS_RES && !HAS_UP), "stem variant");
     static_assert(!MASK || (IN16 && !HAS_UP && !STEM), "mask variant");
+    constexpr bool kTmaEpi = tma_epilogue(HAS_RES, IN16, MASK);
+    static_assert(!kTmaEpi || BLOCK_N <= 128, "residual layers use tiles of at most 128 columns");
     constexpr uint32_t kABytes = BLOCK_M * kRowBytes, kBBytes = BLOCK_N * kRowBytes;
     constexpr int BLOCK_K = IN16 ? 64 : 32;     // elements per K-step
     constexpr uint32_t kStageBytes = kABytes + kBBytes;
+    constexpr uint32_t kResWg = epi_res_bytes(BLOCK_N), kTwinWg = epi_twin_bytes(BLOCK_N);
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
+    uint8_t* epi = smem + kStages * kStageBytes;                  // [2][kResWg] fp32 boxes, then [2][kTwinWg] fp16
+    uint64_t* full = reinterpret_cast<uint64_t*>(epi + (kTmaEpi ? epi_bytes(BLOCK_N) : 0));
     uint64_t* empty = full + kStages;
+    uint64_t* res_full = empty + kStages;     // [2]: the warpgroup's residual boxes have landed
+    uint64_t* res_empty = res_full + 2;       // [2]: its output stores have read the buffer
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const sb_conv_desc& d = p.d;
@@ -99,11 +127,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     if (warp == kProducerWarp && lane == 0) {
         if (!STEM) prefetch_tmap(&map_a);
         prefetch_tmap(&map_b);
+        if (kTmaEpi) prefetch_tmap(&map_r);
         // STEM: a stage is full when the weight tile has landed (1 expect_tx arrival) and the gather threads have
         // written their patch rows.  A stage is empty when every consumer warp's MMAs on it have completed.
         for (int i = 0; i < kStages; ++i) {
             mbar_init(&full[i], STEM ? 1 + 32 * kStemGatherWarps : 1);
             mbar_init(&empty[i], kConsumerWarps);
+        }
+        if (kTmaEpi) {
+            for (int g = 0; g < 2; ++g) {
+                mbar_init(&res_full[g], 1);      // the producer's expect_tx arrival
+                mbar_init(&res_empty[g], 1);     // the warpgroup's store thread
+            }
         }
         fence_barrier_init();
     }
@@ -120,7 +155,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         // ===================== TMA producer =====================
         if (lane == 0) {
             int stage = 0;
-            uint32_t phase = 0;
+            uint32_t phase = 0, rphase = 0;
+            // the tile's residual boxes follow its first min(K-steps, stages) operand loads: those need only free
+            // stages, so they are in flight while the consumers finish the previous tile's epilogue, and the
+            // residual (which waits for that epilogue's stores to leave the buffer) lands during this main loop
+            const int kb_res = (p.num_k_blocks < kStages ? p.num_k_blocks : kStages) - 1;
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
                 const int mt = tile / p.num_n_tiles, nt = tile - mt * p.num_n_tiles;
                 int n_img = 0, h0 = 0, w0 = 0;
@@ -147,6 +186,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                     }
                     tma_load_2d(&map_b, &full[stage], sa + kABytes, tap * d.Cin + c0, nt * BLOCK_N);
                     if (++stage == kStages) { stage = 0; phase ^= 1; }
+                    if (kTmaEpi && kb == kb_res) {
+                        // rows past M and columns past Cout are zero-filled (and still counted in the bytes)
+                        for (int g = 0; g < 2; ++g) {
+                            mbar_wait(&res_empty[g], rphase ^ 1);
+                            mbar_expect_tx(&res_full[g], kResWg);
+                            for (int b = 0; b < BLOCK_N / 32; ++b)
+                                tma_load_2d(&map_r, &res_full[g], epi + g * kResWg + b * kEpiBox, nt * BLOCK_N + 32 * b,
+                                            mt * BLOCK_M + 64 * g);
+                        }
+                        rphase ^= 1;
+                    }
                 }
             }
             if (p.pdl_late) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -248,7 +298,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         const int out_mode = d.out_mode;
         const bool res_biased = d.res_biased != 0;
         int stage = 0;
-        uint32_t phase = 0;
+        uint32_t phase = 0, rphase = 0;
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             const int mt = tile / p.num_n_tiles, nt = tile - mt * p.num_n_tiles;
             int prev = 0;
@@ -277,95 +327,163 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             for (int i = 0; i < kAcc; ++i) reg_fence(acc[i]);
             if (lane == 0) mbar_arrive(&empty[prev]);
 
-            // ---- epilogue: per row {output offset, residual row, upsample source + weights}, then per column pair
-            long long ooff[2];
-            bool valid[2];
-            long long rrow[2];
-            int uoff[2];
-            float uly[2], ulx[2];
-            bool by[2], bx[2];
+            if constexpr (kTmaEpi) {
+                // ---- residual epilogue through shared memory.  The producer has loaded this warpgroup's 64 residual
+                // rows into its fp32 boxes; every thread adds its accumulator pairs to them in place and writes the
+                // fp16 twin beside them, then one thread stores the boxes by TMA (rows past M and columns past Cout
+                // are clipped) and hands the buffer back once the stores have read it.  The global writes drain
+                // while the warpgroup runs the next tile's MMAs.
+                const int rl = 16 * (warp & 3) + (lane >> 2);     // rows rl and rl + 8 of the warpgroup's 64
+                const uint32_t rbuf = smem_u32(epi) + wg * kResWg;
+                const uint32_t tbuf = smem_u32(epi) + 2 * kResWg + wg * kTwinWg;
+                mbar_wait(&res_full[wg], rphase);
+                rphase ^= 1;
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int row = r_lo + 8 * h;
-                int n_img, ho, wo;
-                long long m = 0;
-                if (p.patch) {
-                    const int tw = mt % p.tiles_w;
-                    const int t2 = mt / p.tiles_w;
-                    ho = (t2 % p.tiles_h) * TH + row / TW;
-                    wo = tw * TW + row % TW;
-                    n_img = t2 / p.tiles_h;
-                    valid[h] = ho < d.Ho && wo < d.Wo;
-                } else {
-                    m = (long long)mt * BLOCK_M + row;
-                    valid[h] = m < p.M;
-                    const unsigned mm = valid[h] ? (unsigned)m : 0u;      // M < 2^31 (checked on the host)
-                    const unsigned hw = (unsigned)(d.Ho * d.Wo);
-                    n_img = (int)(mm / hw);
-                    const unsigned rem = mm - (unsigned)n_img * hw;
-                    ho = (int)(rem / (unsigned)d.Wo);
-                    wo = (int)(rem - (unsigned)ho * (unsigned)d.Wo);
-                }
-                ooff[h] = (long long)n_img * d.out_n_stride + (long long)ho * d.out_h_stride +
-                          (long long)wo * d.out_w_stride + d.out_coff;
-                rrow[h] = HAS_RES && valid[h] ? m * d.res_ld : 0;        // (residual: 1x1 convs, flat rows only)
-                uoff[h] = 0; uly[h] = ulx[h] = 0.f; by[h] = bx[h] = false;
-                if (HAS_UP && valid[h]) {
-                    const float sy = __fmul_rn(rh, (float)ho), sx = __fmul_rn(rw, (float)wo);
-                    const int y1 = (int)sy, x1 = (int)sx;
-                    by[h] = y1 < d.UH - 1;
-                    bx[h] = x1 < d.UW - 1;
-                    uoff[h] = (int)((((long long)n_img * d.UH + y1) * d.UW + x1) * d.Cout);
-                    uly[h] = sy - (float)y1;
-                    ulx[h] = sx - (float)x1;
-                }
-            }
+                for (int j = 0; j < BLOCK_N / 8; ++j) {
+                    const int cl = 8 * j + cq;                    // column in the tile
+                    const int c = nt * BLOCK_N + cl;
+                    const int cs = c < d.Cout ? c : 0;            // past Cout: any in-bounds column, never stored
+                    const float2 sc = d.scale ? __ldg(reinterpret_cast<const float2*>(d.scale + cs)) : make_float2(1.f, 1.f);
+                    const float2 sh = d.shift ? __ldg(reinterpret_cast<const float2*>(d.shift + cs)) : make_float2(0.f, 0.f);
 #pragma unroll
-            for (int j = 0; j < BLOCK_N / 8; ++j) {
-                const int c = nt * BLOCK_N + 8 * j + cq;      // Cout % 4 == 0: c < Cout implies c + 1 < Cout
-                if (c >= d.Cout) break;
-                const float2 sc = d.scale ? __ldg(reinterpret_cast<const float2*>(d.scale + c)) : make_float2(1.f, 1.f);
-                const float2 sh = d.shift ? __ldg(reinterpret_cast<const float2*>(d.shift + c)) : make_float2(0.f, 0.f);
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    if (!valid[h]) continue;
-                    float x0 = fmaf(acc[4 * j + 2 * h], sc.x, sh.x);
-                    float x1 = fmaf(acc[4 * j + 2 * h + 1], sc.y, sh.y);
-                    if (HAS_RES) {
-                        float2 r = __ldg(reinterpret_cast<const float2*>(d.residual + rrow[h] + c));
+                    for (int h = 0; h < 2; ++h) {
+                        const uint32_t row = (uint32_t)(rl + 8 * h) * 128;
+                        const uint32_t ra = rbuf + (cl >> 5) * kEpiBox + swz128(row + (cl & 31) * 4);
+                        float2 r = lds64f(ra);
+                        float x0 = fmaf(acc[4 * j + 2 * h], sc.x, sh.x);
+                        float x1 = fmaf(acc[4 * j + 2 * h + 1], sc.y, sh.y);
                         if (res_biased) { r.x = sb_unbias_tf32(r.x); r.y = sb_unbias_tf32(r.y); }
                         x0 += r.x; x1 += r.y;
+                        if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+                        if (out_mode == 1) { x0 = sb_round_tf32(x0); x1 = sb_round_tf32(x1); }
+                        else if (out_mode == 2) { x0 = sb_bias_tf32(x0); x1 = sb_bias_tf32(x1); }
+                        sts64f(ra, x0, x1);
+                        if (d.out16) {   // fp16 twin (round to nearest) for the next tensor-core consumer
+                            if (out_mode == 2) { x0 = sb_unbias_tf32(x0); x1 = sb_unbias_tf32(x1); }
+                            const __half2 hv = __floats2half2_rn(x0, x1);
+                            sts32u(tbuf + (cl >> 6) * kEpiBox + swz128(row + (cl & 63) * 2),
+                                   *reinterpret_cast<const uint32_t*>(&hv));
+                        }
                     }
-                    if (HAS_UP) {
-                        const float* u00 = d.up_src + uoff[h] + c;
-                        const long long dx = bx[h] ? d.Cout : 0;
-                        const long long dy = by[h] ? (long long)d.UW * d.Cout : 0;
-                        const float2 a = __ldg(reinterpret_cast<const float2*>(u00));
-                        const float2 bq = __ldg(reinterpret_cast<const float2*>(u00 + dx));
-                        const float2 g = __ldg(reinterpret_cast<const float2*>(u00 + dy));
-                        const float2 hh = __ldg(reinterpret_cast<const float2*>(u00 + dy + dx));
-                        const float ly1 = uly[h], ly0 = 1.f - ly1, lx1 = ulx[h], lx0 = 1.f - lx1;
-                        x0 += ly0 * (lx0 * a.x + lx1 * bq.x) + ly1 * (lx0 * g.x + lx1 * hh.x);
-                        x1 += ly0 * (lx0 * a.y + lx1 * bq.y) + ly1 * (lx0 * g.y + lx1 * hh.y);
+                }
+                fence_proxy_async();                  // generic-proxy writes -> visible to the TMA stores
+                named_bar_sync(1 + wg, 128);
+                if ((threadIdx.x & 127) == 0) {
+                    const int row0 = mt * BLOCK_M + 64 * wg, col0 = nt * BLOCK_N;
+                    if (row0 < p.M) {
+                        for (int b = 0; d.out && b < BLOCK_N / 32; ++b)
+                            if (col0 + 32 * b < d.Cout) tma_store_2d(&map_o, rbuf + b * kEpiBox, col0 + 32 * b, row0);
+                        for (int b = 0; d.out16 && b < (BLOCK_N + 63) / 64; ++b)
+                            if (col0 + 64 * b < d.Cout) tma_store_2d(&map_o16, tbuf + b * kEpiBox, col0 + 64 * b, row0);
                     }
-                    if (MASK) {
-                        const __half2 mk = *reinterpret_cast<const __half2*>(p.mask16 + ooff[h] + c);
-                        if (!(__low2float(mk) > 0.f)) x0 = 0.f;
-                        if (!(__high2float(mk) > 0.f)) x1 = 0.f;
+                    bulk_commit();
+                    bulk_wait_read<0>();
+                    mbar_arrive(&res_empty[wg]);
+                }
+            } else {
+                // ---- epilogue from registers: per row {output offset, residual row, upsample source + weights}, then
+                // per column pair
+                long long ooff[2];
+                bool valid[2];
+                long long rrow[2];
+                int uoff[2];
+                float uly[2], ulx[2];
+                bool by[2], bx[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int row = r_lo + 8 * h;
+                    int n_img, ho, wo;
+                    long long m = 0;
+                    if (p.patch) {
+                        const int tw = mt % p.tiles_w;
+                        const int t2 = mt / p.tiles_w;
+                        ho = (t2 % p.tiles_h) * TH + row / TW;
+                        wo = tw * TW + row % TW;
+                        n_img = t2 / p.tiles_h;
+                        valid[h] = ho < d.Ho && wo < d.Wo;
+                    } else {
+                        m = (long long)mt * BLOCK_M + row;
+                        valid[h] = m < p.M;
+                        const unsigned mm = valid[h] ? (unsigned)m : 0u;      // M < 2^31 (checked on the host)
+                        const unsigned hw = (unsigned)(d.Ho * d.Wo);
+                        n_img = (int)(mm / hw);
+                        const unsigned rem = mm - (unsigned)n_img * hw;
+                        ho = (int)(rem / (unsigned)d.Wo);
+                        wo = (int)(rem - (unsigned)ho * (unsigned)d.Wo);
                     }
-                    if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-                    if (out_mode == 1) { x0 = sb_round_tf32(x0); x1 = sb_round_tf32(x1); }
-                    else if (out_mode == 2) { x0 = sb_bias_tf32(x0); x1 = sb_bias_tf32(x1); }
-                    if (d.out) *reinterpret_cast<float2*>(d.out + ooff[h] + c) = make_float2(x0, x1);
-                    if (d.out16) {   // fp16 twin (round to nearest) for the next tensor-core consumer
-                        if (out_mode == 2) { x0 = sb_unbias_tf32(x0); x1 = sb_unbias_tf32(x1); }
-                        *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(d.out16) + ooff[h] + c) =
-                            __floats2half2_rn(x0, x1);
+                    ooff[h] = (long long)n_img * d.out_n_stride + (long long)ho * d.out_h_stride +
+                              (long long)wo * d.out_w_stride + d.out_coff;
+                    rrow[h] = HAS_RES && valid[h] ? m * d.res_ld : 0;        // (residual: 1x1 convs, flat rows only)
+                    uoff[h] = 0; uly[h] = ulx[h] = 0.f; by[h] = bx[h] = false;
+                    if (HAS_UP && valid[h]) {
+                        const float sy = __fmul_rn(rh, (float)ho), sx = __fmul_rn(rw, (float)wo);
+                        const int y1 = (int)sy, x1 = (int)sx;
+                        by[h] = y1 < d.UH - 1;
+                        bx[h] = x1 < d.UW - 1;
+                        uoff[h] = (int)((((long long)n_img * d.UH + y1) * d.UW + x1) * d.Cout);
+                        uly[h] = sy - (float)y1;
+                        ulx[h] = sx - (float)x1;
+                    }
+                }
+#pragma unroll
+                for (int j = 0; j < BLOCK_N / 8; ++j) {
+                    const int c = nt * BLOCK_N + 8 * j + cq;      // Cout % 4 == 0: c < Cout implies c + 1 < Cout
+                    const bool cv = c < d.Cout;
+                    const int cs = cv ? c : 0;                    // past Cout: any in-bounds column, never stored
+                    // every load of the column step, for both rows, is issued before its first store (addresses of
+                    // invalid rows and columns are clamped into the tensors instead of branching around the loads)
+                    const float2 sc = d.scale ? __ldg(reinterpret_cast<const float2*>(d.scale + cs)) : make_float2(1.f, 1.f);
+                    const float2 sh = d.shift ? __ldg(reinterpret_cast<const float2*>(d.shift + cs)) : make_float2(0.f, 0.f);
+                    float2 rv[2], ua[2], ub[2], ug[2], uh[2];
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        if (HAS_RES) rv[h] = __ldg(reinterpret_cast<const float2*>(d.residual + rrow[h] + cs));
+                        if (HAS_UP) {
+                            const float* u00 = d.up_src + uoff[h] + cs;
+                            const long long dx = bx[h] ? d.Cout : 0;
+                            const long long dy = by[h] ? (long long)d.UW * d.Cout : 0;
+                            ua[h] = __ldg(reinterpret_cast<const float2*>(u00));
+                            ub[h] = __ldg(reinterpret_cast<const float2*>(u00 + dx));
+                            ug[h] = __ldg(reinterpret_cast<const float2*>(u00 + dy));
+                            uh[h] = __ldg(reinterpret_cast<const float2*>(u00 + dy + dx));
+                        }
+                    }
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        if (!cv || !valid[h]) continue;
+                        float x0 = fmaf(acc[4 * j + 2 * h], sc.x, sh.x);
+                        float x1 = fmaf(acc[4 * j + 2 * h + 1], sc.y, sh.y);
+                        if (HAS_RES) {
+                            float2 r = rv[h];
+                            if (res_biased) { r.x = sb_unbias_tf32(r.x); r.y = sb_unbias_tf32(r.y); }
+                            x0 += r.x; x1 += r.y;
+                        }
+                        if (HAS_UP) {
+                            const float2 a = ua[h], bq = ub[h], g = ug[h], hh = uh[h];
+                            const float ly1 = uly[h], ly0 = 1.f - ly1, lx1 = ulx[h], lx0 = 1.f - lx1;
+                            x0 += ly0 * (lx0 * a.x + lx1 * bq.x) + ly1 * (lx0 * g.x + lx1 * hh.x);
+                            x1 += ly0 * (lx0 * a.y + lx1 * bq.y) + ly1 * (lx0 * g.y + lx1 * hh.y);
+                        }
+                        if (MASK && p.mask16) {     // dgrad without a mask (a residual add only) has mask16 == NULL
+                            const __half2 mk = *reinterpret_cast<const __half2*>(p.mask16 + ooff[h] + c);
+                            if (!(__low2float(mk) > 0.f)) x0 = 0.f;
+                            if (!(__high2float(mk) > 0.f)) x1 = 0.f;
+                        }
+                        if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+                        if (out_mode == 1) { x0 = sb_round_tf32(x0); x1 = sb_round_tf32(x1); }
+                        else if (out_mode == 2) { x0 = sb_bias_tf32(x0); x1 = sb_bias_tf32(x1); }
+                        if (d.out) *reinterpret_cast<float2*>(d.out + ooff[h] + c) = make_float2(x0, x1);
+                        if (d.out16) {   // fp16 twin (round to nearest) for the next tensor-core consumer
+                            if (out_mode == 2) { x0 = sb_unbias_tf32(x0); x1 = sb_unbias_tf32(x1); }
+                            *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(d.out16) + ooff[h] + c) =
+                                __floats2half2_rn(x0, x1);
+                        }
                     }
                 }
             }
             if (tr && threadIdx.x == 0 && tile == (int)blockIdx.x) { tr[4] = gtimer(); tr[12] = clock64(); }
         }
+        if (kTmaEpi && (threadIdx.x & 127) == 0) bulk_wait<0>();     // the last tile's stores have completed
     }
 
     __syncthreads();
@@ -415,9 +533,14 @@ int pick_block_n(int cout, long long m_tiles, int num_sms) {
     return c256 <= c128 ? 256 : 128;
 }
 
+// operands (a, b); residual in, fp32 and fp16 outputs (r, o, o16: the TMA residual epilogue only, zero otherwise)
+struct TcMaps {
+    CUtensorMap a, b, r, o, o16;
+};
+
 template <int BN, int ST, bool RES, bool UP, bool IN16, bool STEM = false, bool MASK = false>
-int launch_t(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& p, cudaStream_t st) {
-    constexpr size_t smem = conv_smem(BN, ST);
+int launch_t(const TcMaps& m, const TcParams& p, cudaStream_t st) {
+    constexpr size_t smem = conv_smem(BN, ST, tma_epilogue(RES, IN16, MASK) ? epi_bytes(BN) : 0);
     static_assert(smem <= 227 * 1024, "smem budget");
     auto kern = conv_tc_kernel<BN, ST, RES, UP, IN16, STEM, MASK>;
     static bool attr_done[kSbMaxDevices] = {false};
@@ -442,30 +565,44 @@ int launch_t(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& p, cu
     attrs[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attrs;
     cfg.numAttrs = use_pdl ? 1 : 0;
-    cudaError_t le = cudaLaunchKernelEx(&cfg, kern, ma, mb, p);
+    cudaError_t le = cudaLaunchKernelEx(&cfg, kern, m.a, m.b, m.r, m.o, m.o16, p);
     SB_LAUNCHED();
     if (le != cudaSuccess) return (int)le;
     SB_CHECK_LAUNCH();
     return SB_OK;
 }
 
-template <int BN, int ST>
-int launch(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& p, cudaStream_t st) {
+// ST: operand stages; ST_RES: operand stages beside the TMA residual epilogue's buffers (0: no such variant)
+template <int BN, int ST, int ST_RES>
+int launch(const TcMaps& m, const TcParams& p, bool dgrad, cudaStream_t st) {
     const bool res = p.d.residual != nullptr, up = p.d.up_src != nullptr;   // never both (supported())
-    if (p.mask16)       // dgrad: fp16 operands, never an upsample source (sb_conv2d_tc_dgrad)
-        return res ? launch_t<BN, ST, true, false, true, false, true>(ma, mb, p, st)
-                   : launch_t<BN, ST, false, false, true, false, true>(ma, mb, p, st);
+    if (dgrad && (p.mask16 || res))     // fp16 operands, never an upsample source (sb_conv2d_tc_dgrad)
+        return res ? launch_t<BN, ST, true, false, true, false, true>(m, p, st)
+                   : launch_t<BN, ST, false, false, true, false, true>(m, p, st);
     if (p.d.in_dtype == 1) {
-        if (up) return launch_t<BN, ST, false, true, true>(ma, mb, p, st);
-        return res ? launch_t<BN, ST, true, false, true>(ma, mb, p, st) : launch_t<BN, ST, false, false, true>(ma, mb, p, st);
+        if (up) return launch_t<BN, ST, false, true, true>(m, p, st);
+        if (res) {
+            if constexpr (ST_RES > 0) return launch_t<BN, ST_RES, true, false, true>(m, p, st);
+            return SB_EINVAL;
+        }
+        return launch_t<BN, ST, false, false, true>(m, p, st);
     }
-    if (up) return launch_t<BN, ST, false, true, false>(ma, mb, p, st);
-    return res ? launch_t<BN, ST, true, false, false>(ma, mb, p, st) : launch_t<BN, ST, false, false, false>(ma, mb, p, st);
+    if (up) return launch_t<BN, ST, false, true, false>(m, p, st);
+    return res ? launch_t<BN, ST, true, false, false>(m, p, st) : launch_t<BN, ST, false, false, false>(m, p, st);
 }
 
-}  // namespace
+// The fp16-operand forward residual epilogue moves the residual and both outputs as 2-D [ld, M] TMA boxes: output
+// pixels must be contiguous rows (m * out_w_stride), and row strides and bases 16-byte aligned.
+bool tma_epilogue_layout_ok(const sb_conv_desc* d) {
+    const long long ws = d->out_w_stride;
+    if (d->Ho > 1 && d->out_h_stride != (long long)d->Wo * ws) return false;
+    if (d->N > 1 && d->out_n_stride != (long long)d->Ho * d->Wo * ws) return false;
+    if (d->out16 && ((ws & 7) || (d->out_coff & 7) || (reinterpret_cast<uintptr_t>(d->out16) & 15))) return false;
+    return true;   // fp32 rows: out_w_stride, out_coff % 4 == 0 and the 16-byte aligned base are checked for every conv
+}
 
-extern "C" int sb_conv2d_tc_supported(const sb_conv_desc* d) {
+// dgrad: the data-gradient entry point, whose residual (and mask) epilogue runs from registers and takes any layout
+int supported(const sb_conv_desc* d, bool dgrad) {
     if (!d || !d->in || !d->wgt) return 0;
     const int bk = d->in_dtype == 1 ? 64 : 32;
     if (d->in_dtype != 0 && d->in_dtype != 1) return 0;
@@ -487,8 +624,13 @@ extern "C" int sb_conv2d_tc_supported(const sb_conv_desc* d) {
     if (d->up_src && ((d->Cout & 3) || (reinterpret_cast<uintptr_t>(d->up_src) & 15))) return 0;
     if (d->Ho != d->H || d->Wo != d->W) return 0;
     if ((long long)d->N * d->Ho * d->Wo >= 0x7fffffffLL) return 0;
+    if (d->residual && d->in_dtype == 1 && !dgrad && !tma_epilogue_layout_ok(d)) return 0;
     return 1;
 }
+
+}  // namespace
+
+extern "C" int sb_conv2d_tc_supported(const sb_conv_desc* d) { return supported(d, false); }
 
 // ---- optional phase trace (tools/conv_trace.py): 16 words per CTA, kTraceCtas CTAs per launch
 namespace {
@@ -516,8 +658,8 @@ extern "C" int sb_conv_trace_info(int id, int* out12) {
 extern "C" int sb_conv_trace_count(void) { return g_trace_n; }
 
 namespace {
-int conv2d_tc(const sb_conv_desc* d, const __half* mask16, sb_stream_t stream) {
-    if (!sb_conv2d_tc_supported(d)) return SB_EINVAL;
+int conv2d_tc(const sb_conv_desc* d, const __half* mask16, bool dgrad, sb_stream_t stream) {
+    if (!supported(d, dgrad)) return SB_EINVAL;
     TcParams p;
     p.d = *d;
     p.mask16 = mask16;
@@ -542,8 +684,10 @@ int conv2d_tc(const sb_conv_desc* d, const __half* mask16, sb_stream_t stream) {
     p.tiles_h = (d->H + TH - 1) / TH;
     p.num_m_tiles = p.patch ? d->N * p.tiles_h * p.tiles_w : (int)((p.M + BLOCK_M - 1) / BLOCK_M);
     int BN = pick_block_n(d->Cout, p.num_m_tiles, sb_num_sms());
-    if (d->residual && BN == 256) BN = 128;   // residual layers are HBM-bound: the narrower tile keeps more CTAs busy
     if (const char* e = getenv("SB_TC_BLOCK_N")) { int v = atoi(e); if ((v == 128 || v == 256) && d->Cout >= 256) BN = v; }
+    // residual layers are HBM-bound: the narrower tile keeps more CTAs busy, and its epilogue buffers fit beside
+    // the operand stages
+    if (d->residual && BN == 256) BN = 128;
     p.num_n_tiles = (d->Cout + BN - 1) / BN;
     if (g_trace && g_trace_n < g_trace_cap) {
         const int id = g_trace_n++;
@@ -553,7 +697,9 @@ int conv2d_tc(const sb_conv_desc* d, const __half* mask16, sb_stream_t stream) {
         v[6] = p.num_k_blocks; v[7] = d->residual ? 1 : 0; v[8] = d->up_src ? 1 : 0; v[9] = 0;
         v[10] = d->max_ctas; v[11] = d->N;
     }
-    CUtensorMap ma, mb;
+    TcMaps m;
+    memset(&m, 0, sizeof(m));
+    CUtensorMap &ma = m.a, &mb = m.b;
     if (p.patch) {
         cuuint64_t dims[4] = {(cuuint64_t)d->Cin, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->N};
         cuuint64_t strides[3] = {(cuuint64_t)d->in_ld * esz, (cuuint64_t)d->W * d->in_ld * esz,
@@ -575,17 +721,30 @@ int conv2d_tc(const sb_conv_desc* d, const __half* mask16, sb_stream_t stream) {
         cuuint32_t box[2] = {(cuuint32_t)BLOCK_K, (cuuint32_t)BN};
         if (!make_map(&mb, d->wgt, 2, dims, strides, box, f16)) return SB_EINVAL;
     }
+    if (d->residual && f16 && !dgrad) {
+        // TMA residual epilogue: [Cout, M] boxes of 64 rows, 32 fp32 / 64 fp16 columns.  A 32-wide tile (Cout <= 32)
+        // stores its twin through a 64-column box whose upper half lies past Cout and is clipped.
+        const cuuint64_t dims[2] = {(cuuint64_t)d->Cout, (cuuint64_t)p.M};
+        const cuuint32_t box32[2] = {32, 64}, box16[2] = {64, 64};
+        const cuuint64_t rs[1] = {(cuuint64_t)d->res_ld * 4};
+        if (!make_map(&m.r, d->residual, 2, dims, rs, box32, false)) return SB_EINVAL;
+        const cuuint64_t os[1] = {(cuuint64_t)d->out_w_stride * 4}, os16[1] = {(cuuint64_t)d->out_w_stride * 2};
+        if (d->out && !make_map(&m.o, d->out + d->out_coff, 2, dims, os, box32, false)) return SB_EINVAL;
+        if (d->out16 && !make_map(&m.o16, reinterpret_cast<const __half*>(d->out16) + d->out_coff, 2, dims, os16,
+                                  box16, true))
+            return SB_EINVAL;
+    }
     cudaStream_t st = sb_cs(stream);
-    switch (BN) {
-        case 32: return launch<32, 9>(ma, mb, p, st);
-        case 64: return launch<64, 8>(ma, mb, p, st);
-        case 256: return launch<256, 4>(ma, mb, p, st);
-        default: return launch<128, 6>(ma, mb, p, st);
+    switch (BN) {        // <BN, operand stages, operand stages beside the residual epilogue buffers>
+        case 32: return launch<32, 9, 9>(m, p, dgrad, st);
+        case 64: return launch<64, 8, 7>(m, p, dgrad, st);
+        case 256: return launch<256, 4, 0>(m, p, dgrad, st);
+        default: return launch<128, 6, 4>(m, p, dgrad, st);
     }
 }
 }  // namespace
 
-extern "C" int sb_conv2d_tc(const sb_conv_desc* d, sb_stream_t stream) { return conv2d_tc(d, nullptr, stream); }
+extern "C" int sb_conv2d_tc(const sb_conv_desc* d, sb_stream_t stream) { return conv2d_tc(d, nullptr, false, stream); }
 
 // Data gradient of a convolution as the forward implicit GEMM on transposed weights (the caller packs them
 // [Cin][kh][kw][Cout], taps flipped, frozen-BN scale folded in), with the ReLU mask of a saved tensor applied after
@@ -593,8 +752,7 @@ extern "C" int sb_conv2d_tc(const sb_conv_desc* d, sb_stream_t stream) { return 
 extern "C" int sb_conv2d_tc_dgrad(const sb_conv_desc* d, const void* mask16, sb_stream_t stream) {
     if (!d || d->in_dtype != 1 || d->up_src || d->relu || d->out_mode != 0) return SB_EINVAL;
     if (reinterpret_cast<uintptr_t>(mask16) & 3) return SB_EINVAL;
-    if (!mask16) return conv2d_tc(d, nullptr, stream);
-    return conv2d_tc(d, reinterpret_cast<const __half*>(mask16), stream);
+    return conv2d_tc(d, reinterpret_cast<const __half*>(mask16), true, stream);
 }
 
 // The stem (resnet.py:111-112: Conv2d(3, 64, 7, stride 2, pad 3) + frozen BN + ReLU) as an implicit GEMM on the tensor
@@ -623,12 +781,13 @@ extern "C" int sb_stem_conv_tc(const float* im_nchw, int N, int H, int W, const 
     p.pdl_late = pdl_late ? 1 : 0;
     p.stem_im = im_nchw; p.sH = H; p.sW = W;
     p.mask16 = nullptr;
-    CUtensorMap mb;
+    TcMaps m;
+    memset(&m, 0, sizeof(m));
     {
         cuuint64_t dims[2] = {192, 64};
         cuuint64_t strides[1] = {192 * 2};
         cuuint32_t box[2] = {64, 64};
-        if (!make_map(&mb, wgt16, 2, dims, strides, box, true)) return SB_EINVAL;
+        if (!make_map(&m.b, wgt16, 2, dims, strides, box, true)) return SB_EINVAL;
     }
-    return launch_t<64, 8, false, false, true, true>(mb, mb, p, sb_cs(stream));
+    return launch_t<64, 8, false, false, true, true>(m, p, sb_cs(stream));
 }

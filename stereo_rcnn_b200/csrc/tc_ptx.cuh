@@ -52,6 +52,27 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* map, uint64_t* ba
         "r"(c2), "r"(c3)
         : "memory");
 }
+// TMA store of a shared-memory box, tracked by the issuing thread's bulk async-group
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t saddr, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(saddr), "r"(c0), "r"(c1)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the source shared memory of all but N committed groups has been read (it may be overwritten)
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() {
+    asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// all but N committed groups have completed (their global writes are done)
+template <int N>
+__device__ __forceinline__ void bulk_wait() {
+    asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+// barrier over `threads` threads (a multiple of 32) on hardware barrier `id` (0 is __syncthreads')
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
@@ -81,5 +102,19 @@ __device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r):
 __device__ __forceinline__ void sts128u(uint32_t saddr, uint4 v) {
     asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
+__device__ __forceinline__ float2 lds64f(uint32_t saddr) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(saddr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void sts64f(uint32_t saddr, float x, float y) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(saddr), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ void sts32u(uint32_t saddr, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(saddr), "r"(v) : "memory");
+}
+// byte offset inside a 1024-byte-aligned region written / read by TMA with 128-byte swizzle: 16-byte chunk
+// (bits 4..6) XOR 128-byte row (bits 7..9)
+__device__ __forceinline__ uint32_t swz128(uint32_t off) { return off ^ (((off >> 7) & 7u) << 4); }
 
 }  // namespace
