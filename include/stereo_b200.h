@@ -155,10 +155,12 @@ typedef struct {
                              * other streams get the remaining SMs) */
 } sb_conv_desc;
 
+/* exact-fp32 SIMT convolution: fp32 operands (in_dtype 0) and the fp32 output only; SB_EINVAL for an fp16
+ * descriptor or a non-NULL out16, before any launch */
 int sb_conv2d_simt(const sb_conv_desc* d, sb_stream_t stream);
 /* tensor-core path: requires Cin % 32 == 0 (K tile = one 128-byte swizzle row), stride 1.  With fp16 operands and a
  * residual, the outputs leave by TMA: output pixels must be contiguous rows (h / n strides = Wo / Ho*Wo pixel
- * strides), and with a twin out_w_stride and out_coff % 8 == 0 and out16 16-byte aligned. */
+ * strides), and with a twin Cout, out_w_stride and out_coff % 8 == 0 and out16 16-byte aligned. */
 int sb_conv2d_tc(const sb_conv_desc* d, sb_stream_t stream);
 int sb_conv2d_tc_supported(const sb_conv_desc* d);
 
@@ -188,7 +190,9 @@ int sb_fpn_grad_combine(const float* dp, const float* dt, int N, int H, int W, i
 
 /* Diagnostics (tools/conv_trace.py): per-CTA phase timestamps of every following sb_conv2d_tc launch, 16 x u64
  * per CTA and 304 CTA slots per launch, into a caller-owned device buffer of sb_conv_trace_bytes(max_launches)
- * bytes.  buf = NULL switches tracing off.  No counterpart in the reference. */
+ * bytes.  buf = NULL switches tracing off.  sb_conv_trace_info(id) gives launch id's {Cin, Cout, kh, M, BLOCK_N, tiles,
+ * K-steps, residual, upsample, variant, max_ctas, N}, variant = 1 (fp16 operands) | 2 (data gradient) | 4 (mask).
+ * No counterpart in the reference. */
 size_t sb_conv_trace_bytes(int max_launches);
 int sb_conv_trace(void* buf, int max_launches);
 int sb_conv_trace_count(void);

@@ -347,6 +347,9 @@ extern "C" int sb_stem_im2col(const float* im_nchw, int N, int H, int W, float* 
 
 extern "C" int sb_conv2d_simt(const sb_conv_desc* d, sb_stream_t stream) {
     if (!d || !d->in || !d->wgt || !d->out) return SB_EINVAL;
+    // fp32 operands and the fp32 output only: an fp16 descriptor would be read as fp32 (past the end of its
+    // buffers) and its twin never written
+    if (d->in_dtype != 0 || d->out16) return SB_EINVAL;
     if (d->Cin % BK != 0 || d->in_ld % 4 != 0) return SB_EINVAL;
     const long long M = (long long)d->N * d->Ho * d->Wo;
     if (M == 0) return SB_OK;

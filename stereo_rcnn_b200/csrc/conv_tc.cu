@@ -592,12 +592,15 @@ int launch(const TcMaps& m, const TcParams& p, bool dgrad, cudaStream_t st) {
 }
 
 // The fp16-operand forward residual epilogue moves the residual and both outputs as 2-D [ld, M] TMA boxes: output
-// pixels must be contiguous rows (m * out_w_stride), and row strides and bases 16-byte aligned.
+// pixels must be contiguous rows (m * out_w_stride), and row strides and bases 16-byte aligned.  The twin's rows must
+// also be a whole number of 16-byte units (Cout % 8 == 0): with Cout = 36 or 100 the bulk tensor store was measured
+// to write fp16 columns past Cout, into the neighbouring channels of a wider row (H100, CUDA 12.9).
 bool tma_epilogue_layout_ok(const sb_conv_desc* d) {
     const long long ws = d->out_w_stride;
     if (d->Ho > 1 && d->out_h_stride != (long long)d->Wo * ws) return false;
     if (d->N > 1 && d->out_n_stride != (long long)d->Ho * d->Wo * ws) return false;
-    if (d->out16 && ((ws & 7) || (d->out_coff & 7) || (reinterpret_cast<uintptr_t>(d->out16) & 15))) return false;
+    if (d->out16 && ((ws & 7) || (d->out_coff & 7) || (d->Cout & 7) || (reinterpret_cast<uintptr_t>(d->out16) & 15)))
+        return false;
     return true;   // fp32 rows: out_w_stride, out_coff % 4 == 0 and the 16-byte aligned base are checked for every conv
 }
 
@@ -694,7 +697,8 @@ int conv2d_tc(const sb_conv_desc* d, const __half* mask16, bool dgrad, sb_stream
         p.trace = g_trace + (size_t)id * kTraceCtas * kTraceWords;
         int* v = g_trace_info[id].v;
         v[0] = d->Cin; v[1] = d->Cout; v[2] = d->kh; v[3] = (int)p.M; v[4] = BN; v[5] = p.num_m_tiles * p.num_n_tiles;
-        v[6] = p.num_k_blocks; v[7] = d->residual ? 1 : 0; v[8] = d->up_src ? 1 : 0; v[9] = 0;
+        v[6] = p.num_k_blocks; v[7] = d->residual ? 1 : 0; v[8] = d->up_src ? 1 : 0;
+        v[9] = (f16 ? 1 : 0) | (dgrad ? 2 : 0) | (mask16 ? 4 : 0);     // operand type and entry point
         v[10] = d->max_ctas; v[11] = d->N;
     }
     TcMaps m;

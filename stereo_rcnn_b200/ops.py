@@ -338,7 +338,7 @@ def conv_desc(x, wgt, out, Cin, Cout, kh, kw, stride, pad, Ho, Wo, scale=None, s
     d.N, d.H, d.W, d.Cin, d.Cout, d.kh, d.kw = N, H, W, Cin, Cout, kh, kw
     d.stride, d.pad, d.Ho, d.Wo = stride, pad, Ho, Wo
     d.in_ld = x.shape[3] if in_ld is None else in_ld
-    d.res_ld = residual.shape[-1] if residual is not None else 0
+    d.res_ld = _flat_rows_ld(residual) if residual is not None else 0
     d.UH, d.UW = (up_src.shape[1], up_src.shape[2]) if up_src is not None else (0, 0)
     d.relu = 1 if relu else 0
     d.out_coff = out_coff
@@ -350,10 +350,27 @@ def conv_desc(x, wgt, out, Cin, Cout, kh, kw, stride, pad, Ho, Wo, scale=None, s
     return d
 
 
+def _flat_rows_ld(t):
+    """row pitch (elements) of an NHWC tensor whose pixels are evenly spaced rows: element (n, h, w, c) at
+    (n*H*W + h*W + w) * ld + c -- the only residual layout the kernels address"""
+    N, H, W, C = t.shape
+    pixels = {0: H * W, 1: W, 2: 1}                  # pixels per step along n, h, w
+    dims = [i for i in (2, 1, 0) if t.shape[i] > 1]  # the stride of a size-1 dimension is arbitrary
+    ld = t.stride(dims[0]) // pixels[dims[0]] if dims else C
+    assert (C == 1 or t.stride(3) == 1) and ld >= C, "residual channels must be contiguous"
+    assert all(t.stride(i) == pixels[i] * ld for i in dims), "residual pixels must be rows of one pitch"
+    return ld
+
+
 def conv2d(desc, impl="auto"):
+    """impl "auto": the tensor-core kernel when it takes the descriptor, else the exact-fp32 SIMT kernel, which
+    has no fp16 mode -- an fp16 descriptor the tensor-core kernel rejects raises"""
     L = _l.load()
     if impl == "auto":
         impl = "tc" if L.sb_conv2d_tc_supported(ctypes.byref(desc)) else "simt"
+        if impl == "simt" and (desc.in_dtype != 0 or desc.out16):
+            raise _l.SbError("sb_conv2d_tc_supported rejects this fp16 descriptor and sb_conv2d_simt has no "
+                             "fp16 mode")
     if impl == "tc":
         check(L.sb_conv2d_tc(ctypes.byref(desc), stream_ptr()), "sb_conv2d_tc")
     else:

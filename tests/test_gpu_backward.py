@@ -53,11 +53,48 @@ WGRAD_CASES = [
     (2, 13, 70, 256, 256, 3),       # 3x3 at 256 (smooth / layer-3 conv2), rows longer than one 64-pixel K-block
     (1, 9, 20, 512, 512, 3),        # 3x3 at 512 (layer-4 conv2)
     (2, 7, 9, 64, 128, 3),          # Cin / Cout not multiples of the 128 tile
+    (2, 5, 7, 256, 64, 1),          # Cout = 64: half of the 128-row dY tile is zero-fill (layer-1 conv1)
+    (2, 6, 9, 64, 64, 3),           # Cin = Cout = 64
+    (1, 1, 1, 64, 128, 1),          # a single pixel: one K-block of 63 zero-filled rows, one bias chunk
+    (1, 1, 1, 128, 64, 3),          # a single pixel, 3x3: eight of nine taps read only the halo
+    (1, 3, 64, 64, 128, 3),         # W = 64: one full 64-pixel chunk per row
+    (1, 3, 65, 128, 64, 3),         # W = 65: a second chunk of one pixel per row
+    (1, 5, 9, 64, 64, 1),           # N*H*W = 45 < 64: fewer pixels than one K-block and than the bias chunks
+    (2, 7, 9, 64, 192, 1),          # Cout = 192: the second m-tile is half empty
 ]
+
+
+def wgrad_plan(N, H, W, Cin, Cout, k, sms):
+    """conv_wgrad.cu plan(): -> (K-blocks, K-blocks per split, splits)"""
+    num_kb = N * H * -(-W // 64) if k == 3 else -(-(N * H * W) // 64)
+    tiles = -(-Cout // 128) * k * k * -(-Cin // 128)
+    splits = max(1, min(-(-2 * sms // tiles), num_kb // 8))
+    kbs = -(-num_kb // splits)
+    return num_kb, kbs, -(-num_kb // kbs)
 
 
 @pytest.mark.parametrize("case", WGRAD_CASES)
 def test_wgrad_exact(case):
+    _check_wgrad(case)
+
+
+@pytest.mark.parametrize("split", ["short_last", "single"])
+def test_wgrad_split_tails(split):
+    """the K-split tails of plan(), found for this device's SM count: a last split shorter than the others (the
+    fixed-order reduction over splits must include it), and a single split"""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    for m in range(64 * 12 + 1, 64 * 400):
+        case = (1, 1, m, 128, 128, 1)
+        num_kb, kbs, splits = wgrad_plan(*case, sms)
+        if m % 64 and (num_kb % kbs and splits > 1 if split == "short_last" else splits == 1 and num_kb > 8):
+            break
+    else:
+        pytest.fail("no shape with a %s split" % split)
+    print("wgrad split %s: M = %d, %d K-blocks, %d per split, %d splits" % (split, m, num_kb, kbs, splits))
+    _check_wgrad(case)
+
+
+def _check_wgrad(case):
     N, H, W, Cin, Cout, k = case
     g = torch.Generator().manual_seed(1)
     dy = torch.randn(N, H, W, Cout, generator=g)
@@ -83,7 +120,13 @@ DGRAD_CASES = [
     (2, 13, 40, 256, 256, 3, 1),
     (1, 9, 20, 512, 512, 3, 1),
     (2, 10, 17, 1024, 256, 1, 1),    # lateral 1x1
+    (1, 5, 13, 64, 256, 1, 1),       # forward Cin = 64: the 64-wide masked variant; M = 65
+    (1, 11, 23, 64, 256, 1, 2),      # ... strided (M = 72 at the strided pixels)
+    (3, 1, 43, 64, 128, 1, 1),       # M = 129: a last m-tile of one row
+    (1, 1, 1, 128, 64, 1, 1),        # a single pixel
+    (1, 9, 17, 64, 64, 3, 1),        # 3x3 patches with a one-row tail
 ]
+SENT32 = 0x7FA5A5A5                  # NaN bit pattern: bytes the data gradient must not write
 
 
 @pytest.mark.parametrize("case", DGRAD_CASES)
@@ -100,7 +143,11 @@ def test_dgrad_exact(case, epi):
     ref = F.conv_transpose2d(nchw(h16(dy)).double(), ws.double(), stride=stride, padding=k // 2,
                              output_padding=(H - 1 - (Ho - 1) * stride))
     ref = ref.permute(0, 2, 3, 1)
-    out = torch.zeros(N, H, W, Cin, device="cuda")
+    # the output inside a sentinel-filled buffer with guard rows: every pixel of the (strided) output written, every
+    # other byte -- the odd positions of a strided scatter included -- left alone
+    lead, n = 5 * Cin, N * H * W * Cin
+    buf = torch.full((lead + n + 7 * Cin,), SENT32, dtype=torch.int32, device="cuda")
+    out = buf[lead:lead + n].view(torch.float32).view(N, H, W, Cin)
     res = mask = None
     if epi == "mask_residual":
         res_cpu = torch.randn(N, Ho, Wo, Cin, generator=g) if k == 1 else None
@@ -116,7 +163,14 @@ def test_dgrad_exact(case, epi):
                     out_strides=(H * W * Cin, stride * W * Cin, stride * Cin))
     G.conv2d_dgrad(d, mask)
     torch.cuda.synchronize()
-    assert l2_err(out, ref) < KERNEL_TOL, l2_err(out, ref)
+    written = torch.zeros(N, H, W, Cin, dtype=torch.bool, device="cuda")
+    written[:, ::stride, ::stride] = True
+    untouched = torch.cat([buf[:lead], buf[lead:lead + n][~written.view(-1)], buf[lead + n:]])
+    assert bool((untouched == SENT32).all()), "bytes outside the data gradient were written"
+    got = out[:, ::stride, ::stride]
+    assert bool(torch.isfinite(got).all()), "elements of the data gradient were not written"
+    ref = ref[:, ::stride, ::stride]
+    assert l2_err(got, ref) < KERNEL_TOL, l2_err(got, ref)
 
 
 @pytest.mark.parametrize("shape", [((2, 38, 125), (2, 19, 63)), ((1, 75, 249), (1, 38, 125)), ((2, 5, 3), (2, 3, 2))])

@@ -76,7 +76,7 @@ def main():
     rows = []
     t_step0 = None
     for i in range(n):
-        cin, cout, kh, M, BN, tiles, kblocks, res, up, small, cap, N = infos[i]
+        cin, cout, kh, M, BN, tiles, kblocks, res, up, variant, cap, N = infos[i]
         live = t[i, :, 0] != 0
         c = t[i, live]
         if c.shape[0] == 0:
@@ -86,7 +86,7 @@ def main():
         if t_step0 is None:
             t_step0 = t0.min()
         rows.append(dict(
-            id=i, cin=cin, cout=cout, k=kh, M=M, N=N, BN=BN, tiles=tiles, kblocks=kblocks, res=res, up=up, small=small,
+            id=i, cin=cin, cout=cout, k=kh, M=M, N=N, BN=BN, tiles=tiles, kblocks=kblocks, res=res, up=up, variant=variant,
             chain=cap, ctas=int(c.shape[0]),
             start_us=(t0.min() - t_step0) / 1e3, first_work_us=(t1.min() - t_step0) / 1e3,
             end_us=(t5.max() - t_step0) / 1e3,
@@ -114,7 +114,8 @@ def main():
     n_sms = float(torch.cuda.get_device_properties(0).multi_processor_count)
     for x in rows:
         key = ("%dx%d" % (x["k"], x["k"])) + ("+res" if x["res"] else "") + ("+up" if x["up"] else "") + \
-              (" flat" if x["small"] == 2 else "") + (" small-M" if x["M"] < 30000 else "")
+              (" f16" if x["variant"] & 1 else " tf32") + (" dgrad" if x["variant"] & 2 else "") + \
+              (" small-M" if x["M"] < 30000 else "")
         c = cls.setdefault(key, [0, 0.0, 0.0, 0.0, 0.0])
         c[0] += 1
         c[1] += x["cta_cyc"] * x["ctas"] / n_sms / clk_mhz
