@@ -16,8 +16,12 @@
 //            CTA builds that strip of the 2x image (one or two rows of it) ONCE in shared memory -- SURVEY 8(d)'s
 //            compulsory traffic: R_rows * (W_span + D_span) pixels per RoI instead of 70 * P gathers;
 //        (c) thread (pixel, hypothesis group) evaluates d = fb / (depth + dz), the bilinear taps out of the strip
-//            (taps outside the strip -- never in practice -- are recomputed from the source) and keeps the SAD of its
-//            13 / 25 hypotheses in registers across rows;
+//            (taps outside the strip are recomputed from the source) and keeps the SAD of its 13 / 25 hypotheses in
+//            registers across rows.  Taps outside the strip are not rare: the coarse depths of a car nearer than
+//            ~12.5 m are clamped to 1.5 m, so some hypotheses have zf + rdis <= 0, d flips sign through the pole and
+//            h = 0 / NH-1 no longer bound the row's reach.  On the 24-RoI golden at 600x1987 (tests/golden/
+//            dense_align.npz), 72 of 691 coarse lattice rows reach over more than kStripMax columns and 33 528 of
+//            2.2 M coarse taps (1.5 %) take the fallback; the fine stage took none there;
 //      then a warp-shuffle + shared-memory reduction to one partial row per CTA.  The fine stage re-derives the
 //      coarse argmin from the partial rows (fixed slice order).
 //   K3 dense_final_kernel: per-RoI argmins, outputs, and the reference's "no valid pixel anywhere ->
@@ -342,7 +346,8 @@ __device__ __forceinline__ void stage_costs(const RoiCtx& g, const Consts& k, co
 // no 152 MB of traffic per call).
 __global__ void __launch_bounds__(256)
 upsample2x_kernel(const float* __restrict__ im0, const float* __restrict__ im1, int H, int W,
-                  float4* __restrict__ up0, float4* __restrict__ up1) {
+                  float4* __restrict__ up0, float4* __restrict__ up1, const int* __restrict__ n_dev) {
+    if (n_dev && *n_dev <= 0) return;        // no live RoI (device-resident count): the pair is never read
     const float* __restrict__ src = blockIdx.z ? im1 : im0;
     float4* __restrict__ dst = blockIdx.z ? up1 : up0;
     const int OH = 2 * H, OW = 2 * W;
@@ -593,7 +598,8 @@ extern "C" int sb_dense_align(const float* im_left, const float* im_right, int H
 }
 
 // D_cap rows are launched; rows >= *n_dev (a device-resident count, e.g. sb_box_solve's n_out) do no work and get no
-// output.  box / pose rows may be wider than 4 / 7 floats (boxes_all [cap,5], poses_all [cap,8] of the solver).
+// output, and with *n_dev == 0 the workspace is not written at all (not even the materialised 2x pair).
+// box / pose rows may be wider than 4 / 7 floats (boxes_all [cap,5], poses_all [cap,8] of the solver).
 extern "C" int sb_dense_align_n(const float* im_left, const float* im_right, int H, int W, const double* calib4,
                                 double scale, const float* box_left, int box_ld, const float* keypoints,
                                 const float* poses, int pose_ld, int D_cap, const int* n_dev, float* status,
@@ -648,7 +654,7 @@ static int dense_align_impl(const float* im_left, const float* im_right, int H, 
     int S = (materialise ? 296 : 592) / D;     // strip kernel: ~4 CTAs per SM (its per-row phases are latency bound)
     if (materialise) {
         dim3 ugrid((k.FW + 255) / 256, k.FH, 2);
-        upsample2x_kernel<<<ugrid, 256, 0, st>>>(im_left, im_right, H, W, upL, upR);
+        upsample2x_kernel<<<ugrid, 256, 0, st>>>(im_left, im_right, H, W, upL, upR, n_dev);
         SB_LAUNCHED();
         SB_CHECK_LAUNCH();
     }

@@ -9,7 +9,6 @@ import torch
 
 from oracle import ops as O
 from stereo_rcnn_b200 import ops as G
-from stereo_rcnn_b200.synth import DEMO_P2, DEMO_P3, gen_rois, synth_pair
 
 pytestmark = pytest.mark.gpu
 
@@ -256,65 +255,6 @@ def test_rpn_head_epilogue_channel_pairing():
     sc = cp.cpu().numpy().reshape(P, 3, 2)[:, :, 1]
     np.testing.assert_allclose(sc, np.stack([s0, s1, s2], 1), rtol=1e-5, atol=1e-7)
     np.testing.assert_array_equal(bp.cpu().numpy().reshape(P, 18), head[0, :, 6:24])
-
-
-# ---------------------------------------------------------------- dense_align
-def test_dense_align_golden(golden_dir):
-    g = np.load(os.path.join(golden_dir, "dense_align.npz"))
-    left, right = synth_pair(int(g["H"]), int(g["W"]), int(g["seed"]), int(g["shift"]))
-    c4 = G.calib_vec(g["p2"], g["p3"])
-    st, dis = G.dense_align(c4, float(g["scale"]), cu(left), cu(right), cu(g["box_left"]), cu(g["keypoints"]),
-                            cu(g["poses"]))
-    np.testing.assert_array_equal(st.cpu().numpy(), g["status"])
-    _check_dense(dis.cpu().numpy(), left, right, c4, float(g["scale"]), g["box_left"], g["keypoints"], g["poses"],
-                 ref_dis=g["best_dis"])
-
-
-def _check_dense(dis, left, right, c4, scale, b, k, p, ref_dis=None):
-    """exact argmin agreement except on photometric near-ties (fp32 sum order), judged on the oracle's costs"""
-    st_o, dis_o, dg = O.dense_align(c4, scale, left, right, b, k, p, diagnostics=True)
-    if ref_dis is not None:
-        np.testing.assert_allclose(dis_o, ref_dis, rtol=1e-6)
-    same = np.abs(dis - dis_o) <= 1e-5 * np.abs(dis_o)
-    assert same.mean() >= 0.97, same.mean()
-    for i in np.nonzero(~same)[0]:
-        cf = dg["cost_fine"][i]
-        cc = dg["cost_coarse"][i]
-        srt = np.sort(cf)
-        src = np.sort(cc)
-        near = (srt[1] - srt[0]) < 1e-4 * srt[0] or (src[1] - src[0]) < 1e-4 * src[0]
-        assert near, (i, dis[i], dis_o[i])
-
-
-@pytest.mark.parametrize("D", [1, 128])
-def test_dense_align_sweep_vs_oracle(D):
-    left, right = synth_pair(600, 1987, 3, 40)
-    b, k, p = gen_rois(D, seed=5)
-    c4 = G.calib_vec(DEMO_P2, DEMO_P3)
-    scale = float(np.float32(1.6))
-    st, dis = G.dense_align(c4, scale, cu(left), cu(right), cu(b), cu(k), cu(p))
-    st_o, _ = O.dense_align(c4, scale, left, right, b, k, p)
-    np.testing.assert_array_equal(st.cpu().numpy(), st_o)
-    _check_dense(dis.cpu().numpy(), left, right, c4, scale, b, k, p)
-
-
-def test_dense_align_no_valid_pixel_early_out_and_module_api():
-    from stereo_rcnn_b200.model.dense_align.dense_align import align_parallel
-
-    class Calib:
-        p2 = np.array([[100., 0, 100, 4], [0, 100., 60, 0], [0, 0, 1, 0]])
-        p3 = np.array([[100., 0, 100, -50], [0, 100., 60, 0], [0, 0, 1, 0]])
-    left, right = synth_pair(120, 200, 5, 4)
-    b = np.array([[5, 5, 30, 30], [6, 6, 28, 33]], np.float32)
-    k = np.array([[17, 1, .9, 5, 30], [17, 1, .9, 6, 28]], np.float32)
-    p = np.array([[30., 1.6, 20., 1.6, 1.5, 3.9, 0.3], [-30., 1.6, 25., 1.6, 1.5, 3.9, 1.0]], np.float32)
-    st, dis = align_parallel(Calib, 1.0, cu(left)[None], cu(right)[None], cu(b), cu(k), cu(p))
-    st_o, dis_o = O.dense_align(O.calib_vec(Calib.p2, Calib.p3), 1.0, left, right, b, k, p)
-    assert st_o.sum() == 0
-    np.testing.assert_array_equal(st.cpu().numpy(), st_o)
-    np.testing.assert_array_equal(dis.cpu().numpy(), dis_o)          # dis_init, bit-exact
-    st, dis = align_parallel(Calib, 1.0, cu(left)[None], cu(right)[None], cu(b[:0]), cu(k[:0]), cu(p[:0]))
-    assert st.numel() == 0 and dis.numel() == 0
 
 
 def test_class_nms_vs_oracle():
