@@ -156,11 +156,11 @@ typedef struct {
 } sb_conv_desc;
 
 /* exact-fp32 SIMT convolution: fp32 operands (in_dtype 0) and the fp32 output only; SB_EINVAL for an fp16
- * descriptor or a non-NULL out16, before any launch */
+ * descriptor, a non-NULL out16 or in_ld < Cin, before any launch */
 int sb_conv2d_simt(const sb_conv_desc* d, sb_stream_t stream);
-/* tensor-core path: requires Cin % 32 == 0 (K tile = one 128-byte swizzle row), stride 1.  With fp16 operands and a
- * residual, the outputs leave by TMA: output pixels must be contiguous rows (h / n strides = Wo / Ho*Wo pixel
- * strides), and with a twin Cout, out_w_stride and out_coff % 8 == 0 and out16 16-byte aligned. */
+/* tensor-core path: requires Cin % 32 == 0 (K tile = one 128-byte swizzle row), in_ld >= Cin, stride 1.  With fp16
+ * operands and a residual, the outputs leave by TMA: output pixels must be contiguous rows (h / n strides = Wo / Ho*Wo
+ * pixel strides), and with a twin Cout, out_w_stride and out_coff % 8 == 0 and out16 16-byte aligned. */
 int sb_conv2d_tc(const sb_conv_desc* d, sb_stream_t stream);
 int sb_conv2d_tc_supported(const sb_conv_desc* d);
 
@@ -201,12 +201,9 @@ int sb_conv_trace_info(int id, int* out12);
 /* stem: NCHW image -> conv7x7/2 + frozen BN + ReLU -> NHWC (resnet.py:111-113) */
 int sb_stem_conv(const float* im_nchw, int N, int H, int W, const float* wgt /*[64][7][7][3]*/,
                  const float* scale, const float* shift, float* out_nhwc, int out_mode, sb_stream_t stream);
-/* stem as a tensor-core GEMM: patch matrix [N*Ho*Wo][160] (k = ci*49+r*7+s, zero padded from 147) that
+/* stem as a TF32 tensor-core GEMM: patch matrix [N*Ho*Wo][160] (k = ci*49+r*7+s, zero padded from 147) that
  * sb_conv2d_tc then multiplies with the [64][160] stem weights (1x1 conv, Cin = 160)              */
 int sb_stem_im2col(const float* im_nchw, int N, int H, int W, float* out, sb_stream_t stream);
-/* fp16 variant: rows of 152 __half (147 taps + 5 zeros; the GEMM multiplies them with [64][192] zero-padded weights,
- * the tensor map zero-fills columns 152..191 of the third 64-wide K-step) */
-int sb_stem_im2col16(const float* im_nchw, int N, int H, int W, void* out_half, sb_stream_t stream);
 /* the stem on the tensor cores with the patch gather INSIDE the GEMM kernel (round 2: no patch matrix in memory):
  * wgt16 = __half [64][192] ((ci, r, s) taps zero padded from 147), out16 = __half NHWC [N,Ho,Wo,64], BN + ReLU fused */
 int sb_stem_conv_tc(const float* im_nchw, int N, int H, int W, const void* wgt16, const float* scale,

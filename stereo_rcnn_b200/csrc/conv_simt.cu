@@ -10,8 +10,6 @@
 // Tile: 128 output pixels x 64 output channels per CTA, K chunks of 16 input channels of
 // one filter tap; 256 threads, 8x4 accumulators each; A/B staged through shared memory
 // with 128-bit global loads, register-prefetched one chunk ahead.
-#include <cuda_fp16.h>
-
 #include "common.cuh"
 
 namespace {
@@ -273,67 +271,7 @@ stem_im2col_kernel(const float* __restrict__ im, int N, int H, int W, int Ho, in
     out[e] = make_float4(v[0], v[1], v[2], v[3]);
 }
 
-// fp16 variant for the f16 GEMM: rows of 192 halves (147 taps, zero padded to 3 K-steps of 64).
-// One CTA = 64 consecutive output pixels of one output row: the 7 x 3 input rows it needs (133 columns
-// each) are staged in shared memory with coalesced loads, then every thread emits 16-byte stores.
-constexpr int kI2cPix = 64;
-constexpr int kI2cGroups = 19;      // 16-byte groups per patch row (152 halves)
-__global__ void __launch_bounds__(256)
-stem_im2col16_kernel(const float* __restrict__ im, int N, int H, int W, int Ho, int Wo, uint4* __restrict__ out) {
-    constexpr int SW = 2 * kI2cPix + 5;            // staged columns
-    __shared__ float tile[3 * 7][SW + 1];
-    const int segs = (Wo + kI2cPix - 1) / kI2cPix;
-    const int seg = blockIdx.x % segs;
-    const int ho = (blockIdx.x / segs) % Ho;
-    const int n = blockIdx.x / (segs * Ho);
-    const int wo0 = seg * kI2cPix;
-    const int wi0 = wo0 * 2 - 3, hi0 = ho * 2 - 3;
-    const float* base = im + (long long)n * 3 * H * W;
-    for (int e = threadIdx.x; e < 21 * SW; e += 256) {
-        const int row = e / SW, col = e - row * SW;
-        const int ci = row / 7, r = row - ci * 7;
-        const int hi = hi0 + r, wi = wi0 + col;
-        float v = 0.f;
-        if (hi >= 0 && hi < H && wi >= 0 && wi < W) v = __ldg(base + ((long long)ci * H + hi) * W + wi);
-        tile[row][col] = v;
-    }
-    __syncthreads();
-    const int npix = min(kI2cPix, Wo - wo0);
-    // rows of 152 halves (19 x 16 B): the 147 taps + 5 zeros.  The GEMM's third K-step reads columns 128..191 through a
-    // tensor map whose inner extent is 152, so TMA zero-fills the rest and 40 of the 192 columns never exist in memory
-    for (int e = threadIdx.x; e < npix * kI2cGroups; e += 256) {
-        const int px = e / kI2cGroups, g = e - px * kI2cGroups;
-        float v[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int k = g * 8 + j;
-            float x = 0.f;
-            if (k < 147) {
-                const int row = k / 7, s2 = k - row * 7;      // row = ci*7 + r
-                x = tile[row][2 * px + s2];
-            }
-            v[j] = x;
-        }
-        __half2 h0 = __floats2half2_rn(v[0], v[1]), h1 = __floats2half2_rn(v[2], v[3]);
-        __half2 h2 = __floats2half2_rn(v[4], v[5]), h3 = __floats2half2_rn(v[6], v[7]);
-        uint4 o;
-        o.x = *reinterpret_cast<uint32_t*>(&h0); o.y = *reinterpret_cast<uint32_t*>(&h1);
-        o.z = *reinterpret_cast<uint32_t*>(&h2); o.w = *reinterpret_cast<uint32_t*>(&h3);
-        out[(((long long)n * Ho + ho) * Wo + wo0 + px) * kI2cGroups + g] = o;
-    }
-}
-
 }  // namespace
-
-extern "C" int sb_stem_im2col16(const float* im_nchw, int N, int H, int W, void* out_half, sb_stream_t stream) {
-    const int Ho = (H + 6 - 7) / 2 + 1, Wo = (W + 6 - 7) / 2 + 1;
-    const long long blocks = (long long)N * Ho * ((Wo + kI2cPix - 1) / kI2cPix);
-    if (blocks <= 0) return SB_EINVAL;
-    stem_im2col16_kernel<<<(unsigned)blocks, 256, 0, sb_cs(stream)>>>(im_nchw, N, H, W, Ho, Wo, (uint4*)out_half);
-    SB_LAUNCHED();
-    SB_CHECK_LAUNCH();
-    return SB_OK;
-}
 
 extern "C" int sb_stem_im2col(const float* im_nchw, int N, int H, int W, float* out, sb_stream_t stream) {
     const int Ho = (H + 6 - 7) / 2 + 1, Wo = (W + 6 - 7) / 2 + 1;
@@ -350,7 +288,7 @@ extern "C" int sb_conv2d_simt(const sb_conv_desc* d, sb_stream_t stream) {
     // fp32 operands and the fp32 output only: an fp16 descriptor would be read as fp32 (past the end of its
     // buffers) and its twin never written
     if (d->in_dtype != 0 || d->out16) return SB_EINVAL;
-    if (d->Cin % BK != 0 || d->in_ld % 4 != 0) return SB_EINVAL;
+    if (d->Cin % BK != 0 || d->in_ld % 4 != 0 || d->in_ld < d->Cin) return SB_EINVAL;
     const long long M = (long long)d->N * d->Ho * d->Wo;
     if (M == 0) return SB_OK;
     dim3 grid(sb_div_up(M, BM), sb_div_up(d->Cout, BN));

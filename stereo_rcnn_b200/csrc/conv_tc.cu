@@ -65,7 +65,6 @@ struct TcParams {
     int kblocks_per_tap;  // Cin / BLOCK_K
     int num_k_blocks;     // taps * kblocks_per_tap
     long long M;
-    int pdl_late;         // fire griddepcontrol.launch_dependents after the last operand loads instead of at entry
     unsigned long long* trace;   // optional per-CTA phase timestamps (sb_conv_trace), 16 words per CTA
     // STEM variant: the A operand is gathered from the NCHW fp32 image [N,3,sH,sW] (7x7 / stride 2 / pad 3 patches)
     const float* stem_im;
@@ -144,8 +143,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     }
     __syncthreads();
     // Programmatic dependent launch: everything above (barrier init, descriptor prefetch) overlapped the previous
-    // kernel's tail.  Let the next kernel start its own prologue, then wait for the producers of our activations.
-    if (!p.pdl_late) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    // kernel's tail.  Wait for the producers of our activations; the producer warp releases the next kernel below.
     asm volatile("griddepcontrol.wait;" ::: "memory");
     if (tr && threadIdx.x == 0) { tr[1] = gtimer(); tr[9] = clock64(); }
 
@@ -199,7 +197,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                     }
                 }
             }
-            if (p.pdl_late) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+            // release the dependent launch once this CTA's last operand loads are issued: an earlier release lets the
+            // next kernel's CTAs sit in griddepcontrol.wait on SMs the other stream's chain could be using
+            asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
             if (tr) { tr[3] = gtimer(); tr[11] = clock64(); }
         }
     } else if (STEM && warp > kProducerWarp) {
@@ -554,7 +554,6 @@ int launch_t(const TcMaps& m, const TcParams& p, cudaStream_t st) {
     int slots = sb_num_sms();
     if (p.d.max_ctas > 0 && p.d.max_ctas < slots) slots = p.d.max_ctas;
     const int grid = tiles < slots ? tiles : slots;
-    static const bool use_pdl = getenv("SB_NO_PDL") == nullptr;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(STEM ? kStemThreads : kThreads);
@@ -564,7 +563,7 @@ int launch_t(const TcMaps& m, const TcParams& p, cudaStream_t st) {
     attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attrs[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attrs;
-    cfg.numAttrs = use_pdl ? 1 : 0;
+    cfg.numAttrs = 1;
     cudaError_t le = cudaLaunchKernelEx(&cfg, kern, m.a, m.b, m.r, m.o, m.o16, p);
     SB_LAUNCHED();
     if (le != cudaSuccess) return (int)le;
@@ -610,6 +609,7 @@ int supported(const sb_conv_desc* d, bool dgrad) {
     const int bk = d->in_dtype == 1 ? 64 : 32;
     if (d->in_dtype != 0 && d->in_dtype != 1) return 0;
     if (d->stride != 1 || d->Cin % bk != 0 || d->in_ld % (d->in_dtype == 1 ? 8 : 4) != 0) return 0;
+    if (d->in_ld < d->Cin) return 0;      // a shorter row would read the next pixel's channels (past the end on the last)
     if (!d->out && !d->out16) return 0;
     const bool k1 = d->kh == 1 && d->kw == 1 && d->pad == 0;
     const bool k3 = d->kh == 3 && d->kw == 3 && d->pad == 1;
@@ -666,10 +666,6 @@ int conv2d_tc(const sb_conv_desc* d, const __half* mask16, bool dgrad, sb_stream
     TcParams p;
     p.d = *d;
     p.mask16 = mask16;
-    // default: release the dependent launch once this CTA's last operand loads are issued -- an early release lets
-    // the next kernel's CTAs sit in griddepcontrol.wait on SMs the other stream's chain could be using
-    static const bool pdl_late = getenv("SB_PDL_LATE") == nullptr || atoi(getenv("SB_PDL_LATE")) != 0;
-    p.pdl_late = pdl_late ? 1 : 0;
     p.trace = nullptr;
     p.stem_im = nullptr;
     p.sH = p.sW = 0;
@@ -711,9 +707,7 @@ int conv2d_tc(const sb_conv_desc* d, const __half* mask16, bool dgrad, sb_stream
         cuuint32_t box[4] = {(cuuint32_t)BLOCK_K, TW, TH, 1};
         if (!make_map(&ma, d->in, 4, dims, strides, box, f16)) return SB_EINVAL;
     } else {
-        // a row may be SHORTER than Cin (in_ld < Cin: the stem's 152-wide patch rows under a 192-wide zero-padded weight):
-        // the map's inner extent is then the row length and TMA zero-fills the rest of the last K-step
-        cuuint64_t dims[2] = {(cuuint64_t)(d->in_ld < d->Cin ? d->in_ld : d->Cin), (cuuint64_t)p.M};
+        cuuint64_t dims[2] = {(cuuint64_t)d->Cin, (cuuint64_t)p.M};
         cuuint64_t strides[1] = {(cuuint64_t)d->in_ld * esz};
         cuuint32_t box[2] = {(cuuint32_t)BLOCK_K, BLOCK_M};
         if (!make_map(&ma, d->in, 2, dims, strides, box, f16)) return SB_EINVAL;
@@ -781,8 +775,6 @@ extern "C" int sb_stem_conv_tc(const float* im_nchw, int N, int H, int W, const 
     if (p.M >= 0x7fffffffLL || p.M * 64 >= 0x7fffffffLL) return SB_EINVAL;
     p.num_m_tiles = (int)((p.M + BLOCK_M - 1) / BLOCK_M); p.num_n_tiles = 1;
     p.kblocks_per_tap = 3; p.num_k_blocks = 3;
-    static const bool pdl_late = getenv("SB_PDL_LATE") == nullptr || atoi(getenv("SB_PDL_LATE")) != 0;
-    p.pdl_late = pdl_late ? 1 : 0;
     p.stem_im = im_nchw; p.sH = H; p.sW = W;
     p.mask16 = nullptr;
     TcMaps m;

@@ -18,7 +18,6 @@
 //      channel-vector loads), then averaged and stored as coalesced channel vectors -- the
 //      lattice (69 MB for the 14x14 keypoint pooling) never touches HBM.
 #include <cuda_fp16.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 
@@ -344,9 +343,7 @@ extern "C" int sb_roi_align_pyramid_nhwc(const float* const* feats, const int* h
         a.scale[l] = (float)((double)heights[l] / (double)im_h);
     }
     // output rows per CTA: all of a 7x7 tile (8 lattice rows for 7 outputs), half of a 14x14 tile
-    int RB = pooled <= 8 ? pooled : (pooled + 1) / 2;
-    static const int rb_env = getenv("SB_ROI_RB") ? atoi(getenv("SB_ROI_RB")) : 0;     // A/B knob (tools/ab.sh)
-    if (rb_env > 0) RB = rb_env < pooled ? rb_env : pooled;
+    const int RB = pooled <= 8 ? pooled : (pooled + 1) / 2;
     size_t smem = (size_t)2 * (pooled + 1) * C * sizeof(float) + (size_t)(RB + 1) * (pooled + 1) * sizeof(TapRec);
     if (smem > 200 * 1024) return SB_EINVAL;
     static size_t cur_max_dev[kSbMaxDevices] = {0};

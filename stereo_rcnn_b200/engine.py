@@ -80,32 +80,26 @@ class PackedConv(object):
 class StereoRCNNEngine(object):
     """state_dict uses the reference's key names (RCNN_layer1.0.0.conv1.weight, ...)"""
 
-    def __init__(self, state_dict, device="cuda", n_classes=2, conv_impl="auto", precision=None, lr_streams=None):
+    def __init__(self, state_dict, device="cuda", n_classes=2, conv_impl="auto", precision=None, forks=True):
         """precision: "tf32" (fp32 storage, tf32) or "fp16" (fp16 conv operands, f16, fp32 accumulate
         and fp32 residual stream); default from $SB_PRECISION, else "fp16" (same measured accuracy as tf32 --
-        both round operands to an 11-bit significand -- at twice the MMA rate and half the activation bytes).  conv_impl="simt" forces exact fp32."""
+        both round operands to an 11-bit significand -- at twice the MMA rate and half the activation bytes).  conv_impl="simt" forces exact fp32.
+        forks=True is the latency schedule: layers 3-4 of the left and the right image run as two concurrent chains,
+        and the coarse RPN levels and the box head run on a side stream beside the rest.  forks=False is the
+        throughput schedule, one chain with no forks: with several independent pairs in flight the SMs are already
+        full and the batched chain (fewer, wider tiles) costs less SM time."""
         import os
         precision = precision or os.environ.get("SB_PRECISION", "fp16")
         assert precision in ("tf32", "fp16")
         self.half = precision == "fp16" and conv_impl != "simt"
         self.precision = "fp32-simt" if conv_impl == "simt" else precision
         self.keep32 = False
-        self.chain_ctas = int(os.environ.get("SB_CHAIN_CTAS", "0"))
-        self.stem_fused = os.environ.get("SB_STEM_FUSED", "1") != "0"
-        self.rpn_streams = os.environ.get("SB_RPN_STREAMS", "1") != "0"
-        self.head_streams = os.environ.get("SB_HEAD_STREAMS", "1") != "0"
-        # lr_streams: run layers 3-4 of the left and the right image as two concurrent chains (lowest latency of a
-        # single pair).  With several independent pairs in flight the SMs are already full and the batched chain
-        # (fewer, wider tiles) costs less SM time: callers that pipeline pairs pass lr_streams=False.
-        if lr_streams is None:
-            lr_streams = os.environ.get("SB_LR_STREAMS", "1") != "0"
-        self.lr_streams = bool(lr_streams)
+        self.forks = bool(forks)
         self.side = torch.cuda.Stream(device=torch.device(device)) if torch.device(device).type == "cuda" else None
         self.device = torch.device(device)
         self.n_classes = n_classes
         self.conv_impl = conv_impl
         self.impl_used = {}
-        self.max_ctas = 0         # grid cap for convs issued while a second chain runs on the side stream
         self.record = None        # bench: list collecting (desc, live tensors) of every conv launch of a forward
         # conv_impl="simt" is the exact-fp32 yardstick: exact weights, exact stores, no TF32 hygiene modes
         self.exact = conv_impl == "simt"
@@ -144,9 +138,6 @@ class StereoRCNNEngine(object):
         wst = torch.zeros(64, 160, 1, 1)                              # stem as a GEMM over the padded patch matrix
         wst[:, :147, 0, 0] = sd["RCNN_layer0.0.weight"].reshape(64, 147)      # (ci, r, s) order of sb_stem_im2col
         self.p["stem_gemm"] = PackedConv(wst, s, b, 0)
-        wst = torch.zeros(64, 192, 1, 1)                              # fp16 variant: three 64-wide K-steps
-        wst[:, :147, 0, 0] = sd["RCNN_layer0.0.weight"].reshape(64, 147)
-        self.p["stem_gemm16"] = PackedConv(wst, s, b, 0)
         self.stem_w16 = ops.pack_stem_w16(sd["RCNN_layer0.0.weight"])   # K layout of the fused (implicit-GEMM) stem
         for li, nb in enumerate(LAYERS):
             for bi in range(nb):
@@ -194,7 +185,7 @@ class StereoRCNNEngine(object):
 
     # ------------------------------------------------------------------ helpers
     def _conv(self, x, pc, relu=False, stride=1, residual=None, up_src=None, out=None, out_coff=0,
-              out_strides=None, Cin=None, tag=None, out_mode=ops.EXACT, res_biased=False, in_biased=False,
+              out_strides=None, tag=None, out_mode=ops.EXACT, res_biased=False, in_biased=False,
               f32=True, f16=False, out16=None):
         """x fp32 (tf32 / simt modes) or fp16 (fp16 mode).  Returns the fp32 output, the fp16 twin, or both."""
         N, H, W = x.shape[:3]
@@ -207,10 +198,10 @@ class StereoRCNNEngine(object):
             out16 = torch.empty(N, Ho, Wo, pc.Cout, dtype=torch.float16, device=x.device)
         if self.exact or half_in:
             out_mode, res_biased, in_biased = ops.EXACT, False, False
-        d = ops.conv_desc(x, pc.w16 if half_in else pc.w, out, pc.Cin if Cin is None else Cin, pc.Cout, pc.kh,
+        d = ops.conv_desc(x, pc.w16 if half_in else pc.w, out, pc.Cin, pc.Cout, pc.kh,
                           pc.kw, stride, pc.pad, Ho, Wo, scale=pc.scale, shift=pc.shift, residual=residual,
                           up_src=up_src, relu=relu, out_coff=out_coff, out_strides=out_strides, out_mode=out_mode,
-                          res_biased=res_biased, in_biased=in_biased, out16=out16, max_ctas=self.max_ctas)
+                          res_biased=res_biased, in_biased=in_biased, out16=out16)
         impl = ops.conv2d(d, "tc" if half_in else self.conv_impl)
         if self.record is not None:
             self.record.append((d, impl, (x, out, out16, residual, up_src)))
@@ -287,12 +278,9 @@ class StereoRCNNEngine(object):
         """fp16-operand trunk: every conv input is an fp16 tensor (half the HBM bytes, f16 = 2x the TF32
         MMA rate, same 11-bit significand); fp32 copies exist only where a non-conv consumer needs them
         (residual adds, FPN upsample source, RoIAlign, the user-visible P levels)."""
-        if self.stem_fused:     # patches gathered inside the GEMM kernel: no 229 MB patch matrix
-            pc = self.p["stem_gemm16"]
-            c0 = ops.stem_conv_tc(im_nchw, self.stem_w16, pc.scale, pc.shift)
-            self.impl_used["stem"] = "tc16-fused"
-        else:
-            c0 = self._conv(ops.stem_im2col16(im_nchw), self.p["stem_gemm16"], relu=True, tag="stem", f32=False, f16=True)
+        # patches gathered inside the GEMM kernel (no 229 MB patch matrix); self.stem[1:] is the folded BN scale, shift
+        c0 = ops.stem_conv_tc(im_nchw, self.stem_w16, *self.stem[1:])
+        self.impl_used["stem"] = "tc16-fused"
         c1 = ops.maxpool3x3s2_ceil(c0)
         feats = {"c1": c1.float() if self.keep32 else None, "c1_16": c1}
         saved = {} if save_for_backward else None
@@ -328,14 +316,12 @@ class StereoRCNNEngine(object):
                     y32, y16 = self._bottleneck16(y32, y16, "RCNN_layer%d.0.%d" % (li + 1, bi),
                                                   STRIDES[li] if bi == 0 else 1, bi == 0,
                                                   out=(dst[0][sl], dst[1][sl]) if last else None, saved=saved)
-        if self.side is not None and self.lr_streams and saved is None:
+        if self.side is not None and self.forks and saved is None:
             main = torch.cuda.current_stream()
             self.side.wait_stream(main)
-            self.max_ctas = self.chain_ctas      # each chain keeps to half of the SMs so that both really co-run
             with torch.cuda.stream(self.side):
                 chain(slice(B, N))
             chain(slice(0, B))
-            self.max_ctas = 0
             main.wait_stream(self.side)
         else:
             chain(slice(0, N))
@@ -476,7 +462,7 @@ class StereoRCNNEngine(object):
         offs = [0]
         for h, w in shapes:
             offs.append(offs[-1] + h * w)
-        fork = self.side is not None and self.rpn_streams
+        fork = self.side is not None and self.forks
         if fork:    # the three coarse levels are a handful of tiles each: run them beside the p2 / p3 convs
             main = torch.cuda.current_stream()
             self.side.wait_stream(main)
@@ -509,7 +495,7 @@ class StereoRCNNEngine(object):
                            out_mode=ops.ROUND_TF32, **c16)
             fc7 = self._conv(x, self.p["RCNN_top.3"], relu=True, tag="top3").view(R, 2048)
             return (pooled, fc7) + tuple(ops.box_tail(fc7, *self.fc, n_classes=self.n_classes))
-        fork = self.side is not None and self.head_streams
+        fork = self.side is not None and self.forks
         if fork:    # the box head (two FCs with 3 row tiles) is latency-bound: run it beside the keypoint convs
             main = torch.cuda.current_stream()
             self.side.wait_stream(main)

@@ -92,7 +92,6 @@ _SIGS = {
     "sb_stem_conv": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "sb_stem_im2col": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "sb_stem_conv_tc": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "sb_stem_im2col16": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "sb_maxpool3x3s2_ceil16": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "sb_maxpool3x3s2_ceil": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "sb_subsample2": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),

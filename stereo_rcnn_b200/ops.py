@@ -319,7 +319,7 @@ def kitti_result_lines(final, t_cam2_cam0_x):
 
 # ------------------------------------------------------------- layer ops ----
 def conv_desc(x, wgt, out, Cin, Cout, kh, kw, stride, pad, Ho, Wo, scale=None, shift=None, residual=None,
-              up_src=None, relu=False, in_ld=None, out_coff=0, out_strides=None, out_mode=0, res_biased=False,
+              up_src=None, relu=False, out_coff=0, out_strides=None, out_mode=0, res_biased=False,
               in_biased=False, out16=None, max_ctas=0):
     """x: NHWC [N,H,W,in_ld]; wgt packed [Cout,kh,kw,Cin]; out: any tensor addressed through out_strides
     = (n, h, w) strides in floats (default: dense NHWC of out.shape[-1] channels)."""
@@ -337,7 +337,7 @@ def conv_desc(x, wgt, out, Cin, Cout, kh, kw, stride, pad, Ho, Wo, scale=None, s
     d.up_src = up_src.data_ptr() if up_src is not None else None
     d.N, d.H, d.W, d.Cin, d.Cout, d.kh, d.kw = N, H, W, Cin, Cout, kh, kw
     d.stride, d.pad, d.Ho, d.Wo = stride, pad, Ho, Wo
-    d.in_ld = x.shape[3] if in_ld is None else in_ld
+    d.in_ld = x.shape[3]
     d.res_ld = _flat_rows_ld(residual) if residual is not None else 0
     d.UH, d.UW = (up_src.shape[1], up_src.shape[2]) if up_src is not None else (0, 0)
     d.relu = 1 if relu else 0
@@ -451,17 +451,6 @@ def stem_im2col(im_nchw):
     Ho, Wo = (H + 6 - 7) // 2 + 1, (W + 6 - 7) // 2 + 1
     out = torch.empty(N, Ho, Wo, 160, dtype=torch.float32, device=im_nchw.device)
     check(L.sb_stem_im2col(ptr(_f32c(im_nchw)), N, H, W, ptr(out), stream_ptr()), "sb_stem_im2col")
-    return out
-
-
-def stem_im2col16(im_nchw):
-    """-> fp16 [N, Ho, Wo, 152] patch matrix of the stem (147 taps + 5 zeros; the GEMM's tensor map zero-fills up to
-    the 192 columns of its zero-padded weights)"""
-    L = _l.load()
-    N, _, H, W = im_nchw.shape
-    Ho, Wo = (H + 6 - 7) // 2 + 1, (W + 6 - 7) // 2 + 1
-    out = torch.empty(N, Ho, Wo, 152, dtype=torch.float16, device=im_nchw.device)
-    check(L.sb_stem_im2col16(ptr(_f32c(im_nchw)), N, H, W, ptr(out), stream_ptr()), "sb_stem_im2col16")
     return out
 
 

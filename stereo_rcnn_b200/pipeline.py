@@ -10,8 +10,6 @@ with no host synchronisation, so that it can be captured into a CUDA graph and r
                             workspaces (ops.WorkspaceOwner) and the CUDA graph of one step.  Several slots may
                             replay concurrently; they share nothing but the (read-only) weights.
 """
-import os
-
 import numpy as np
 import torch
 
@@ -25,13 +23,10 @@ class StereoPipeline(object):
         """throughput=True: the schedule for several pairs in flight -- no intra-pair stream forks (left/right
         chains, RPN levels, box head): they shorten one pair's latency but cost SM time that other pairs can use"""
         self.dev = torch.device(device)
-        self.eng = engine.StereoRCNNEngine(state_dict, device, lr_streams=False if throughput else None,
-                                           precision=precision)
-        if throughput and os.environ.get("SB_TP_FORKS", "0") == "0":
-            self.eng.rpn_streams = self.eng.head_streams = False
+        self.eng = engine.StereoRCNNEngine(state_dict, device, precision=precision, forks=not throughput)
         self.scale = float(np.float32(scale))
         self._info = {}
-        self.side = torch.cuda.Stream(device=self.dev) if os.environ.get("SB_SIDE_STREAM", "1") != "0" else None
+        self.side = torch.cuda.Stream(device=self.dev)
 
     def im_info(self, B, H, W):
         key = (B, H, W)
@@ -57,7 +52,7 @@ class StereoPipeline(object):
             with torch.cuda.stream(self.side):
                 for b in range(B):
                     side_out.append(ops.dense_align(calib4, self.scale, iml[b], imr[b], *rois3d[b]))
-        o = self.eng.forward(iml, imr, info, before_proposals=fork_dense_align if self.side is not None else None)
+        o = self.eng.forward(iml, imr, info, before_proposals=fork_dense_align)
         R = o["rois_left"].shape[1]
         if record is None:
             record = torch.empty(B, R, parallel.REC_COLS, dtype=torch.float32, device=self.dev)
@@ -70,11 +65,7 @@ class StereoPipeline(object):
                 o["kpts_prob"][sl], o["left_border_prob"][sl], o["right_border_prob"][sl], info[b],
                 n_classes=N_CLASSES, record=record[b])
             ops.class_nms(o["cls_prob"][b], pbl, 1, 0.05, 0.3, keep=keep[b], num=nkeep[b:b + 1])
-        if self.side is not None:
-            torch.cuda.current_stream().wait_stream(self.side)
-        else:
-            for b in range(B):
-                side_out.append(ops.dense_align(calib4, self.scale, iml[b], imr[b], *rois3d[b]))
+        torch.cuda.current_stream().wait_stream(self.side)
         st = [s for s, _d in side_out]
         dis = [d for _s, d in side_out]
         return record, keep, nkeep, st, dis

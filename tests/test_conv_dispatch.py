@@ -65,6 +65,11 @@ CASES = [
     ("in_ld_f16_8", desc(Cin=64, in_ld=72), True),
     ("in_ld_tf32_not4", desc(f16=False, Cin=32, in_ld=34), False),
     ("in_ld_tf32_4", desc(f16=False, Cin=32, in_ld=36), True),
+    # rows at least Cin wide: a shorter row would read the next pixel's channels
+    ("in_ld_short_f16", desc(Cin=128, in_ld=120), False),
+    ("in_ld_full_f16", desc(Cin=128, in_ld=128), True),
+    ("in_ld_short_tf32", desc(f16=False, Cin=64, in_ld=60), False),
+    ("in_ld_full_tf32", desc(f16=False, Cin=64, in_ld=64), True),
     ("no_outputs", desc(out=None, twin=False), False),
     ("twin_only", desc(out=None), True),
     ("fp32_only", desc(twin=False), True),
@@ -156,6 +161,12 @@ def test_simt_rejects_fp16_descriptors_before_launch(lib):
     with SB_EINVAL (-22) before any launch (no device is needed to get the answer)"""
     for d in (desc(), rows(desc(res=True)), desc(f16=False, Cin=32, twin=True), desc(out=None)):
         assert lib.sb_conv2d_simt(ctypes.byref(d), None) == -22
+
+
+def test_simt_rejects_short_rows_before_launch(lib):
+    """an fp32 descriptor whose input rows are narrower than Cin is refused with SB_EINVAL before any launch"""
+    d = desc(f16=False, Cin=32, in_ld=28)
+    assert lib.sb_conv2d_simt(ctypes.byref(d), None) == -22
 
 
 def test_auto_dispatch_raises_for_rejected_fp16(lib):

@@ -360,9 +360,10 @@ def test_reference_module_interface(golden_dir):
         m.train()
 
 
-def test_latency_and_throughput_schedules_agree():
-    """The latency schedule (left/right chains of layers 3-4, RPN levels and the box head forked onto a second
-    stream; narrower tiles for the per-image chains) and the throughput schedule (one batched chain, no forks)
+def test_forked_and_unforked_schedules_agree():
+    """The latency schedule (forks=True: left/right chains of layers 3-4, RPN levels and the box head forked onto a
+    second stream; narrower tiles for the per-image chains) and the throughput schedule (forks=False: one batched
+    chain, no forks)
     launch the same arithmetic: a conv output element is the same K-ordered wgmma accumulation whatever the tile
     width, so features agree to rounding noise at most and the proposals are identical."""
     H, W = 160, 320
@@ -371,10 +372,8 @@ def test_latency_and_throughput_schedules_agree():
     iml, imr = cu(torch.from_numpy(left)[None]), cu(torch.from_numpy(right)[None])
     info = cu(torch.tensor([[float(H), float(W), 1.0]]))
     outs = []
-    for lr in (True, False):
-        eng = E.StereoRCNNEngine(sd, "cuda", lr_streams=lr)
-        if not lr:
-            eng.rpn_streams = eng.head_streams = False
+    for forks in (True, False):
+        eng = E.StereoRCNNEngine(sd, "cuda", forks=forks)
         o = eng.forward(iml, imr, info, keep_features=True)
         torch.cuda.synchronize()
         outs.append(o)

@@ -36,9 +36,7 @@ def main():
     left, right = synth_pair(H, W, 3, 48)
     im = torch.cat((torch.from_numpy(left)[None], torch.from_numpy(right)[None]), 0).cuda().contiguous()
     info = torch.tensor([[H, W, 1.6]], device="cuda")
-    eng = engine.StereoRCNNEngine(make_state_dict(3), "cuda", lr_streams=False if a.throughput else None)
-    if a.throughput:
-        eng.rpn_streams = eng.head_streams = False
+    eng = engine.StereoRCNNEngine(make_state_dict(3), "cuda", forks=not a.throughput)
 
     def fwd():
         feats = eng.trunk_fpn(im)
@@ -76,7 +74,7 @@ def main():
     rows = []
     t_step0 = None
     for i in range(n):
-        cin, cout, kh, M, BN, tiles, kblocks, res, up, variant, cap, N = infos[i]
+        cin, cout, kh, M, BN, tiles, kblocks, res, up, variant, _max_ctas, N = infos[i]
         live = t[i, :, 0] != 0
         c = t[i, live]
         if c.shape[0] == 0:
@@ -87,7 +85,7 @@ def main():
             t_step0 = t0.min()
         rows.append(dict(
             id=i, cin=cin, cout=cout, k=kh, M=M, N=N, BN=BN, tiles=tiles, kblocks=kblocks, res=res, up=up, variant=variant,
-            chain=cap, ctas=int(c.shape[0]),
+            ctas=int(c.shape[0]),
             start_us=(t0.min() - t_step0) / 1e3, first_work_us=(t1.min() - t_step0) / 1e3,
             end_us=(t5.max() - t_step0) / 1e3,
             span_us=(t5.max() - t0.min()) / 1e3, work_span_us=(t5.max() - t1.min()) / 1e3,
@@ -100,10 +98,10 @@ def main():
     with open(a.out, "w") as f:
         json.dump(dict(step_ms=step_ms, launches=rows), f)
     print("graph step %.3f ms, %d traced conv launches" % (step_ms, len(rows)))
-    print(" id  cin cout k      M  BN tiles ctas ch | start   work0     end |  span  wspan  wait | fill   mma  epi1  tail   cta ctamax (cycles) skew_us")
+    print(" id  cin cout k      M  BN tiles ctas | start   work0     end |  span  wspan  wait | fill   mma  epi1  tail   cta ctamax (cycles) skew_us")
     for x in rows:
-        print("%3d %4d %4d %d %6d %3d %5d %4d %2d | %6.1f %6.1f %6.1f | %5.1f %5.1f %5.1f | %5.0f %5.0f %5.0f %5.0f %6.0f %6.0f  %5.1f" % (
-            x["id"], x["cin"], x["cout"], x["k"], x["M"], x["BN"], x["tiles"], x["ctas"], 1 if x["chain"] else 0,
+        print("%3d %4d %4d %d %6d %3d %5d %4d | %6.1f %6.1f %6.1f | %5.1f %5.1f %5.1f | %5.0f %5.0f %5.0f %5.0f %6.0f %6.0f  %5.1f" % (
+            x["id"], x["cin"], x["cout"], x["k"], x["M"], x["BN"], x["tiles"], x["ctas"],
             x["start_us"], x["first_work_us"], x["end_us"], x["span_us"], x["work_span_us"], x["wait_us"],
             x["fill_cyc"], x["mma_cyc"], x["epi1_cyc"], x["tail_cyc"], x["cta_cyc"], x["cta_cyc_max"], x["start_skew_us"]))
 

@@ -35,8 +35,11 @@ def main():
     b, k, p = (torch.from_numpy(x).cuda() for x in gen_rois(32, seed=3))
     c4 = ops.calib_vec(DEMO_P2, DEMO_P3)
 
+    def stem():
+        return ops.stem_conv_tc(im, eng.stem_w16, *eng.stem[1:])
+
     def trunk_only():
-        c0 = eng._conv(ops.stem_im2col16(im), eng.p["stem_gemm16"], relu=True, f32=False, f16=True)
+        c0 = stem()
         c1 = ops.maxpool3x3s2_ceil(c0)
         x32, x16 = None, c1
         outs = []
@@ -47,8 +50,8 @@ def main():
             outs.append((x32, x16))
         return outs
     t_layers = []
-    t, _ = timed_graph(lambda: eng._conv(ops.stem_im2col16(im), eng.p["stem_gemm16"], relu=True, f32=False, f16=True))
-    print("stem (im2col + GEMM)      %7.3f ms" % t)
+    t, _ = timed_graph(stem)
+    print("stem (fused gather+GEMM)  %7.3f ms" % t)
     t_tr, _ = timed_graph(trunk_only)
     print("stem + layers 1-4         %7.3f ms" % t_tr)
     t_tf, feats = timed_graph(lambda: eng.trunk_fpn(im))
