@@ -53,7 +53,9 @@ int sb_nms_mask(const float* dets, int n, float thresh, uint64_t* mask, sb_strea
 
 /* ----------------------------------------------------------- RoIAlign ----
  * Reference semantics: features NCHW fp32, rois R x 5 [batch,x1,y1,x2,y2],
- * (ah, aw) is the tap lattice (RoIAlignAvg passes pooled+1), out R x C x ah x aw. */
+ * (ah, aw) is the tap lattice (RoIAlignAvg passes pooled+1), out R x C x ah x aw.
+ * SB_EINVAL unless H >= 2 and W >= 2 (the bilinear cell at hstart = min(floor(h), H-2)
+ * must lie inside the map).                                                          */
 int sb_roi_align_forward(const float* features, int N, int C, int H, int W,
                          const float* rois, int R, int ah, int aw, float spatial_scale,
                          float* out, sb_stream_t stream);
@@ -76,7 +78,16 @@ int sb_roi_align_backward_det(const float* top_grad, int N, int C, int H, int W,
 /* Fused PyramidRoI_Feat: level routing (Q14) + per-level scale (Q15) + tap lattice +
  * 2x2/stride-1 average, NHWC features, one launch for all levels.
  * feats[l]: N x H_l x W_l x C (l = P2..P5); out[r][ph][pw][out_coff + c], row pitch out_ld elements;
- * round_tf32: 0 = exact fp32, 1 = fp32 rounded to TF32, 2 = __half output (out is then a __half*). */
+ * round_tf32: 0 = exact fp32, 1 = fp32 rounded to TF32, 2 = __half output (out is then a __half*).
+ * SB_EINVAL, before any launch, unless: R >= 0; C > 0 and C % 4 == 0; pooled >= 1; out_ld % 4 == 0;
+ * out_coff >= 0, out_coff % 4 == 0 and out_coff + C <= out_ld; round_tf32 in {0, 1, 2}; every level
+ * has a non-null pointer and H_l >= 2, W_l >= 2; rois and out non-null when R > 0; and the kernel's
+ * shared memory, 8 (pooled+1) C + 40 (rb+1)(pooled+1) bytes with rb = pooled <= 8 ? pooled : (pooled+1)/2,
+ * is at most 200 KB.  R == 0 launches nothing.
+ * Mode 0 is bit-exact with the reference's arithmetic (fp32 lattice values rounded once from fp64, the
+ * 2x2 average in fp32) except where an fp64 lattice value lies within ~2^-50 of an fp32 rounding tie;
+ * modes 1 and 2 are mode 0 rounded (TF32 ties away, fp16 ties to even).  The level, round(logf(..) + 4),
+ * may differ from a correctly rounded log's for a RoI within 1 ulp of a level boundary. */
 int sb_roi_align_pyramid_nhwc(const float* const* feats, const int* heights, const int* widths,
                               int C, float im_h, const float* rois, int R, int pooled,
                               float* out, int out_ld, int out_coff, int round_tf32, sb_stream_t stream);

@@ -276,7 +276,8 @@ extern "C" int sb_roi_align_forward(const float* features, int N, int C, int H, 
                                     sb_stream_t stream) {
     (void)N;
     if (R == 0) return SB_OK;
-    if (R < 0 || C <= 0 || ah < 2 || aw < 2 || !features || !rois || !out) return SB_EINVAL;
+    // H, W >= 2: hstart = min(floor(h), H-2) must be a row of the map for every tap inside it
+    if (R < 0 || C <= 0 || H < 2 || W < 2 || ah < 2 || aw < 2 || !features || !rois || !out) return SB_EINVAL;
     dim3 grid(R, (C + 31) / 32);
     roi_align_fwd_nchw<<<grid, 256, 0, sb_cs(stream)>>>(features, C, H, W, rois, ah, aw, spatial_scale, out);
     SB_LAUNCHED();
@@ -289,7 +290,7 @@ extern "C" int sb_roi_align_backward(const float* top_grad, int N, int C, int H,
                                      sb_stream_t stream) {
     (void)N;
     if (R == 0) return SB_OK;
-    if (R < 0 || C <= 0 || ah < 2 || aw < 2 || !top_grad || !rois || !bottom_grad) return SB_EINVAL;
+    if (R < 0 || C <= 0 || H < 2 || W < 2 || ah < 2 || aw < 2 || !top_grad || !rois || !bottom_grad) return SB_EINVAL;
     dim3 grid(R, (C + 31) / 32);
     roi_align_bwd_nchw<<<grid, 256, 0, sb_cs(stream)>>>(top_grad, C, H, W, rois, ah, aw, spatial_scale, bottom_grad);
     SB_LAUNCHED();
@@ -332,8 +333,16 @@ extern "C" int sb_roi_align_pyramid_nhwc(const float* const* feats, const int* h
                                          int C, float im_h, const float* rois, int R, int pooled,
                                          float* out, int out_ld, int out_coff, int round_tf32,
                                          sb_stream_t stream) {
+    // every check before the first CUDA call: a rejected call neither launches nor touches the device.  The output
+    // slice [out_coff, out_coff + C) must lie inside its row, and each level must have two rows and two columns
+    // (hstart = min(floor(h), H-2) is a row of the map only then).
+    if (R < 0 || C <= 0 || (C & 3) || pooled < 1 || (out_ld & 3) || out_coff < 0 || (out_coff & 3) ||
+        (long long)out_coff + C > out_ld || round_tf32 < 0 || round_tf32 > 2 || !feats || !heights || !widths)
+        return SB_EINVAL;
+    for (int l = 0; l < 4; ++l)
+        if (!feats[l] || heights[l] < 2 || widths[l] < 2) return SB_EINVAL;
     if (R == 0) return SB_OK;
-    if (R < 0 || (C & 3) || pooled < 1 || (out_ld & 3) || (out_coff & 3)) return SB_EINVAL;
+    if (!rois || !out) return SB_EINVAL;
     PyramidArgs a;
     for (int l = 0; l < 4; ++l) {
         a.feat[l] = feats[l];

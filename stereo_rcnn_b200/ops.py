@@ -144,7 +144,12 @@ def roi_align_pyramid_nhwc(feats, im_h, rois, pooled, out=None, out_coff=0, roun
     """feats: 4 NHWC fp32 tensors (P2..P5); rois [R,5]; -> out [R,pooled,pooled,out_ld] NHWC (fp32, fp32 rounded
     to TF32, or fp16 when half=True)"""
     L = _l.load()
+    assert len(feats) == 4
     C = feats[0].shape[3]
+    for f in feats:       # the kernel reads each level as dense [N, H, W, C] fp32 rows on the RoIs' device
+        assert f.dim() == 4 and f.dtype == torch.float32 and f.is_contiguous() and f.shape[3] == C, \
+            "pyramid levels must be contiguous fp32 NHWC tensors with the same C"
+        assert f.device == rois.device, "pyramid levels must be on the RoIs' device"
     R = rois.shape[0]
     if out is None:
         out = torch.empty(R, pooled, pooled, C, dtype=torch.float16 if half else torch.float32, device=rois.device)

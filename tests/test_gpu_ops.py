@@ -179,26 +179,6 @@ def test_roi_align_backward_deterministic_fixed_point():
     assert float(g2.abs().max()) == 0.0
 
 
-@pytest.mark.parametrize("pooled", [7, 14])
-def test_roi_align_pyramid_nhwc_vs_oracle(pooled):
-    rs = np.random.RandomState(11)
-    shapes = [(150, 497), (75, 249), (38, 125), (19, 63)]
-    C = 64
-    feats = [rs.randn(1, C, h, w).astype(np.float32) for h, w in shapes]
-    R = 120
-    x1 = rs.rand(R) * 1500
-    y1 = rs.rand(R) * 400
-    side = np.exp(rs.uniform(np.log(8), np.log(900), R))
-    rois = np.stack([np.zeros(R), x1, y1, np.minimum(x1 + side * rs.uniform(0.5, 2, R), 1986),
-                     np.minimum(y1 + side, 599)], 1).astype(np.float32)
-    rois[0] = 0
-    ref = O.pyramid_roi_feat(feats, rois, 600.0, pooled)             # R,C,p,p
-    assert len(set(O.roi_levels(rois).tolist())) == 4
-    fd = [cu(f.transpose(0, 2, 3, 1)) for f in feats]
-    out = G.roi_align_pyramid_nhwc(fd, 600.0, cu(rois), pooled).cpu().numpy().transpose(0, 3, 1, 2)
-    np.testing.assert_allclose(out, ref, rtol=1e-5, atol=1e-5)
-
-
 # ------------------------------------------------------------- proposal layer
 def test_proposal_layer_golden_bit_exact(golden_dir):
     g = np.load(os.path.join(golden_dir, "proposal_small.npz"))
