@@ -121,6 +121,9 @@ int sb_generate_anchors(const sb_proposal_cfg* cfg, int A, float* anchors, sb_st
  * with the reference's softmax channel pairing (stereo_rpn.py:52-60,81-83)               */
 int sb_rpn_head_epilogue(const float* head, int B, int P, int ld, float* cls_prob, float* bbox_pred,
                          sb_stream_t stream);
+/* the raw class scores the RPN loss reads (stereo_rpn.py:89,116-119: rpn_cls_score, each pixel's six score channels as
+ * the consecutive pairs (c0,c1), (c2,c3), (c4,c5)): head [B, P, ld] -> rpn_cls_score [B, 3P, 2]; ld >= 6 */
+int sb_rpn_head_scores(const float* head, int B, int P, int ld, float* rpn_cls_score, sb_stream_t stream);
 
 /* -------------------------------------------------------- dense_align ----
  * im_left/right: 3 x H x W planar fp32 (network-scale, batch 1).
@@ -198,6 +201,27 @@ int sb_conv_wgrad(const void* dy16, const void* x16, int N, int H, int W, int Ci
                   void* workspace, size_t workspace_bytes, sb_stream_t stream);
 int sb_fpn_grad_combine(const float* dp, const float* dt, int N, int H, int W, int TH, int TW, int C,
                         const float* dp6, int H6, int W6, float scale, float* out, void* out16, sb_stream_t stream);
+
+/* ------------------------------------------------- backward pass of the stereo RPN (fp16 operands, fp32 accumulate) ----
+ * Together these replace the autograd of lib/model/rpn/stereo_rpn.py:73-95 (RPN_Conv, RPN_cls_score,
+ * RPN_bbox_pred_left_right) that loss.backward() runs in trainval_net.py.
+ * sb_rpn_head_grad -- gradient of the fused RPN head's output from the sb_rpn_loss gradients d_cls_score [B,A,2] and
+ *   d_bbox_pred [B,A,6] (A = 3P): dhead16 [B,P,64] fp16 = grad_scale * d in columns 0..5 (the raw scores' channels) and
+ *   6..23 (the 18 box channels), zero in 24..63; dhead32 (may be NULL) its fp32 twin.  No softmax: the loss reads the
+ *   raw scores.
+ * sb_conv_wgrad_acc -- sb_conv_wgrad on strided operands with accumulation: pixel p of dy16 / x16 / dy32 starts at
+ *   element p * dy_ld / x_ld / dy32_ld (dy_ld, x_ld multiples of 8, >= Cout / Cin; dy16, x16 16-byte aligned).
+ *   accumulate != 0 adds the results to dw / db (stream order, so a fixed call order gives bit-identical sums).
+ *   Rows co < split of dW / db go to dw / db, rows split <= co < rows to dw_hi / db_hi (row co - split), rows >= rows
+ *   are not stored (1 <= split <= rows <= Cout).  With dense strides, accumulate = 0 and split = rows = Cout the results
+ *   are bit-identical to sb_conv_wgrad's.  Workspace of sb_conv_wgrad_acc_workspace bytes.                        */
+int sb_rpn_head_grad(const float* d_cls_score, const float* d_bbox_pred, int B, int P, float grad_scale,
+                     void* dhead16, float* dhead32, sb_stream_t stream);
+size_t sb_conv_wgrad_acc_workspace(int N, int H, int W, int Cin, int Cout, int k);
+int sb_conv_wgrad_acc(const void* dy16, int dy_ld, const void* x16, int x_ld, int N, int H, int W, int Cin, int Cout,
+                      int k, const float* scale, float inv_grad_scale, const float* dy32, int dy32_ld, int accumulate,
+                      int rows, int split, float* dw, float* db, float* dw_hi, float* db_hi, int* nonfinite,
+                      void* workspace, size_t workspace_bytes, sb_stream_t stream);
 
 /* Diagnostics (tools/conv_trace.py): per-CTA phase timestamps of every following sb_conv2d_tc launch, 16 x u64
  * per CTA and 304 CTA slots per launch, into a caller-owned device buffer of sb_conv_trace_bytes(max_launches)

@@ -11,6 +11,10 @@
 //     folded frozen-BN scale s[cout], divides out the gradient scale and writes the reference layout
 //     [Cout][Cin][kh][kw].  Bias gradients are column sums of the fp32 dY, also two-level in a fixed order.
 //     No float atomics: results are bit-identical run to run.  A non-finite gradient sets *nonfinite = 1.
+//   * sb_conv_wgrad_acc: the same GEMM on strided operands (dY may be a channel slice of a wider tensor), with the
+//     results optionally added to the destination in stream order -- a sum over several convs that share one weight
+//     (the RPN conv over five levels and two images) stays bit-identical run to run -- and the rows of dW / db split
+//     over two destinations (the fused RPN head holds the reference's two 1x1 convs).
 //   * sb_fpn_grad_combine: the gradient of one FPN level,
 //       dP = scale * dP_in + up^T(dT) + scatter2(scale * dP6)
 //     where up^T is the transpose of the align_corners bilinear upsample of stereo_rcnn.py:91-108 (a gather over the
@@ -166,12 +170,26 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_const
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
 
-// second pass: dW[co][ci][r][s] = s[co] / grad_scale * sum over splits (ascending) of the partial tiles
-__global__ void wgrad_reduce_kernel(const float* __restrict__ part, WgParams p, int Cin, int Cout,
-                                    const float* __restrict__ scale, float inv_scale, float* __restrict__ dw,
-                                    int* nonfinite) {
+// second pass: dW[co][ci][r][s] = s[co] / grad_scale * sum over splits (ascending) of the partial tiles.  Rows
+// co < o.split go to o.dw, rows o.split <= co < o.rows to o.dw_hi (row co - split), rows past o.rows are dropped;
+// o.accumulate adds the result to what the destination holds.
+struct WgOut {
+    float *dw, *dw_hi, *db, *db_hi;
+    int rows, split, accumulate;
+};
+
+__device__ __forceinline__ void store_row_value(float* lo, float* hi, int split, int co, size_t row_elems, size_t i,
+                                                float v, int accumulate, int* nonfinite) {
+    float* dst = co < split ? lo + (size_t)co * row_elems + i : hi + (size_t)(co - split) * row_elems + i;
+    if (accumulate) v = *dst + v;
+    *dst = v;
+    if (nonfinite && !isfinite(v)) *nonfinite = 1;
+}
+
+__global__ void wgrad_reduce_kernel(const float* __restrict__ part, WgParams p, int Cin, WgOut o,
+                                    const float* __restrict__ scale, float inv_scale, int* nonfinite) {
     const int taps = p.k * p.k;
-    const long long total = (long long)Cout * Cin * taps;
+    const long long total = (long long)o.rows * Cin * taps;
     const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= total) return;
     const int co = (int)(e / ((long long)Cin * taps));
@@ -182,32 +200,29 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ part, WgParams p, 
     const size_t sstride = (size_t)p.tiles * (kWgBM * kWgBN);
     float acc = 0.f;
     for (int s = 0; s < p.splits; ++s) acc += __ldg(src + s * sstride);
-    float v = acc * (scale ? __ldg(scale + co) : 1.f) * inv_scale;
-    dw[e] = v;
-    if (nonfinite && !isfinite(v)) *nonfinite = 1;
+    const float v = acc * (scale ? __ldg(scale + co) : 1.f) * inv_scale;
+    store_row_value(o.dw, o.dw_hi, o.split, co, (size_t)Cin * taps, rem, v, o.accumulate, nonfinite);
 }
 
-// bias gradient, first level: partial[chunk][c] = sum of rows [chunk*rows, ...) of dy[M][C] (ascending)
-__global__ void colsum_partial_kernel(const float* __restrict__ dy, long long M, int C, long long rows,
+// bias gradient, first level: partial[chunk][c] = sum of rows [chunk*rows, ...) of dy[M][C] (row pitch ld, ascending)
+__global__ void colsum_partial_kernel(const float* __restrict__ dy, long long M, int C, long long ld, long long rows,
                                       float* __restrict__ partial) {
     const long long r0 = (long long)blockIdx.x * rows;
     const long long r1 = min(M, r0 + rows);
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
         float acc = 0.f;
-        for (long long r = r0; r < r1; ++r) acc += __ldg(dy + r * C + c);
+        for (long long r = r0; r < r1; ++r) acc += __ldg(dy + r * ld + c);
         partial[(size_t)blockIdx.x * C + c] = acc;
     }
 }
 
-__global__ void colsum_final_kernel(const float* __restrict__ partial, int chunks, int C, float inv_scale,
-                                    float* __restrict__ db, int* nonfinite) {
+__global__ void colsum_final_kernel(const float* __restrict__ partial, int chunks, int C, float inv_scale, WgOut o,
+                                    int* nonfinite) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= C) return;
+    if (c >= o.rows) return;
     float acc = 0.f;
     for (int i = 0; i < chunks; ++i) acc += partial[(size_t)i * C + c];
-    const float v = acc * inv_scale;
-    db[c] = v;
-    if (nonfinite && !isfinite(v)) *nonfinite = 1;
+    store_row_value(o.db, o.db_hi, o.split, c, 1, 0, acc * inv_scale, o.accumulate, nonfinite);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -254,40 +269,45 @@ size_t part_bytes(const WgParams& p) { return (size_t)p.splits * p.tiles * kWgBM
 
 int bias_chunks(long long M) { return (int)min((long long)kBiasChunks, M); }
 
-}  // namespace
-
-extern "C" size_t sb_conv_wgrad_workspace(int N, int H, int W, int Cin, int Cout, int k) {
+size_t wgrad_workspace(int N, int H, int W, int Cin, int Cout, int k) {
     if (N < 1 || H < 1 || W < 1 || Cin < 1 || Cout < 1 || (k != 1 && k != 3)) return 0;
     const WgParams p = plan(N, H, W, Cin, Cout, k);
     return part_bytes(p) + (size_t)kBiasChunks * Cout * sizeof(float) + 256;
 }
 
-extern "C" int sb_conv_wgrad(const void* dy16, const void* x16, int N, int H, int W, int Cin, int Cout, int k,
-                             const float* scale, float inv_grad_scale, float* dw, const float* dy32, float* db,
-                             int* nonfinite, void* workspace, size_t workspace_bytes, sb_stream_t stream) {
-    if (!dy16 || !x16 || !dw || N < 1 || H < 1 || W < 1 || (k != 1 && k != 3)) return SB_EINVAL;
-    if (Cin % 64 || Cout % 64 || (db && !dy32)) return SB_EINVAL;
-    if ((reinterpret_cast<uintptr_t>(dy16) & 15) || (reinterpret_cast<uintptr_t>(x16) & 15) ||
-        (reinterpret_cast<uintptr_t>(workspace) & 15))
+bool misaligned(const void* q, uintptr_t a) { return (reinterpret_cast<uintptr_t>(q) & (a - 1)) != 0; }
+
+// dy16 / x16 / dy32 rows (pixels) are dy_ld / x_ld / dy32_ld elements apart; every argument is checked before the
+// first launch
+int conv_wgrad(const void* dy16, int dy_ld, const void* x16, int x_ld, int N, int H, int W, int Cin, int Cout, int k,
+               const float* scale, float inv_grad_scale, const float* dy32, int dy32_ld, WgOut o, int* nonfinite,
+               void* workspace, size_t workspace_bytes, cudaStream_t st) {
+    if (!dy16 || !x16 || !o.dw || N < 1 || H < 1 || W < 1 || (k != 1 && k != 3)) return SB_EINVAL;
+    if (Cin < 64 || Cout < 64 || Cin % 64 || Cout % 64 || (o.db && !dy32)) return SB_EINVAL;
+    if (dy_ld < Cout || x_ld < Cin || dy_ld % 8 || x_ld % 8 || (dy32 && dy32_ld < Cout)) return SB_EINVAL;
+    if (o.rows < 1 || o.rows > Cout || o.split < 1 || o.split > o.rows || (o.split < o.rows && !o.dw_hi) ||
+        (o.db && o.split < o.rows && !o.db_hi))
         return SB_EINVAL;
-    if (workspace_bytes < sb_conv_wgrad_workspace(N, H, W, Cin, Cout, k)) return SB_EINVAL;
+    if (misaligned(dy16, 16) || misaligned(x16, 16) || misaligned(workspace, 16) || misaligned(dy32, 4))
+        return SB_EINVAL;
+    if (workspace_bytes < wgrad_workspace(N, H, W, Cin, Cout, k)) return SB_EINVAL;
     const long long M = (long long)N * H * W;
     if (M >= 0x7fffffffLL) return SB_EINVAL;
     WgParams p = plan(N, H, W, Cin, Cout, k);
     p.part = reinterpret_cast<float*>(workspace);
-    cudaStream_t st = sb_cs(stream);
 
     CUtensorMap mdy, mx;
+    const cuuint64_t yl = (cuuint64_t)dy_ld * 2, xl = (cuuint64_t)x_ld * 2;
     if (p.patch) {
         cuuint64_t dd[4] = {(cuuint64_t)Cout, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-        cuuint64_t ds[3] = {(cuuint64_t)Cout * 2, (cuuint64_t)W * Cout * 2, (cuuint64_t)H * W * Cout * 2};
+        cuuint64_t ds[3] = {yl, W * yl, (cuuint64_t)H * W * yl};
         cuuint64_t xd[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-        cuuint64_t xs[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)W * Cin * 2, (cuuint64_t)H * W * Cin * 2};
+        cuuint64_t xs[3] = {xl, W * xl, (cuuint64_t)H * W * xl};
         cuuint32_t box[4] = {64, (cuuint32_t)kWgBK, 1, 1};
         if (!make_map16(&mdy, dy16, 4, dd, ds, box) || !make_map16(&mx, x16, 4, xd, xs, box)) return SB_EINVAL;
     } else {
-        cuuint64_t dd[2] = {(cuuint64_t)Cout, (cuuint64_t)M}, ds[1] = {(cuuint64_t)Cout * 2};
-        cuuint64_t xd[2] = {(cuuint64_t)Cin, (cuuint64_t)M}, xs[1] = {(cuuint64_t)Cin * 2};
+        cuuint64_t dd[2] = {(cuuint64_t)Cout, (cuuint64_t)M}, ds[1] = {yl};
+        cuuint64_t xd[2] = {(cuuint64_t)Cin, (cuuint64_t)M}, xs[1] = {xl};
         cuuint32_t box[2] = {64, (cuuint32_t)kWgBK};
         if (!make_map16(&mdy, dy16, 2, dd, ds, box) || !make_map16(&mx, x16, 2, xd, xs, box)) return SB_EINVAL;
     }
@@ -301,23 +321,50 @@ extern "C" int sb_conv_wgrad(const void* dy16, const void* x16, int N, int H, in
     conv_wgrad_kernel<<<p.tiles * p.splits, kWgThreads, kWgSmem, st>>>(mdy, mx, p);
     SB_LAUNCHED();
     SB_CHECK_LAUNCH();
-    const long long total = (long long)Cout * Cin * k * k;
-    wgrad_reduce_kernel<<<sb_div_up(total, 256), 256, 0, st>>>(p.part, p, Cin, Cout, scale, inv_grad_scale, dw,
-                                                                nonfinite);
+    const long long total = (long long)o.rows * Cin * k * k;
+    wgrad_reduce_kernel<<<sb_div_up(total, 256), 256, 0, st>>>(p.part, p, Cin, o, scale, inv_grad_scale, nonfinite);
     SB_LAUNCHED();
     SB_CHECK_LAUNCH();
-    if (db) {
+    if (o.db) {
         float* bp = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + part_bytes(p));
         const int chunks = bias_chunks(M);
         const long long rows = (M + chunks - 1) / chunks;
-        colsum_partial_kernel<<<chunks, 256, 0, st>>>(dy32, M, Cout, rows, bp);
+        colsum_partial_kernel<<<chunks, 256, 0, st>>>(dy32, M, Cout, dy32_ld, rows, bp);
         SB_LAUNCHED();
         SB_CHECK_LAUNCH();
-        colsum_final_kernel<<<sb_div_up(Cout, 256), 256, 0, st>>>(bp, chunks, Cout, inv_grad_scale, db, nonfinite);
+        colsum_final_kernel<<<sb_div_up(o.rows, 256), 256, 0, st>>>(bp, chunks, Cout, inv_grad_scale, o, nonfinite);
         SB_LAUNCHED();
         SB_CHECK_LAUNCH();
     }
     return SB_OK;
+}
+
+}  // namespace
+
+extern "C" size_t sb_conv_wgrad_workspace(int N, int H, int W, int Cin, int Cout, int k) {
+    return wgrad_workspace(N, H, W, Cin, Cout, k);
+}
+
+extern "C" int sb_conv_wgrad(const void* dy16, const void* x16, int N, int H, int W, int Cin, int Cout, int k,
+                             const float* scale, float inv_grad_scale, float* dw, const float* dy32, float* db,
+                             int* nonfinite, void* workspace, size_t workspace_bytes, sb_stream_t stream) {
+    const WgOut o = {dw, nullptr, db, nullptr, Cout, Cout, 0};
+    return conv_wgrad(dy16, Cout, x16, Cin, N, H, W, Cin, Cout, k, scale, inv_grad_scale, dy32, Cout, o, nonfinite,
+                      workspace, workspace_bytes, sb_cs(stream));
+}
+
+extern "C" size_t sb_conv_wgrad_acc_workspace(int N, int H, int W, int Cin, int Cout, int k) {
+    return wgrad_workspace(N, H, W, Cin, Cout, k);
+}
+
+extern "C" int sb_conv_wgrad_acc(const void* dy16, int dy_ld, const void* x16, int x_ld, int N, int H, int W, int Cin,
+                                 int Cout, int k, const float* scale, float inv_grad_scale, const float* dy32,
+                                 int dy32_ld, int accumulate, int rows, int split, float* dw, float* db, float* dw_hi,
+                                 float* db_hi, int* nonfinite, void* workspace, size_t workspace_bytes,
+                                 sb_stream_t stream) {
+    const WgOut o = {dw, dw_hi, db, db_hi, rows, split, accumulate ? 1 : 0};
+    return conv_wgrad(dy16, dy_ld, x16, x_ld, N, H, W, Cin, Cout, k, scale, inv_grad_scale, dy32, dy32_ld, o,
+                      nonfinite, workspace, workspace_bytes, sb_cs(stream));
 }
 
 // ------------------------------------------------------------------ FPN level gradient

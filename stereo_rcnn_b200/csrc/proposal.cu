@@ -16,6 +16,7 @@
 //      reduction with on-the-fly intersection and early exit at post_nms_top_n
 //   6. gather + zero padding into rois_left / rois_right
 // Memory-bound: reads scores (A*8 B) 4x from L2, deltas only for survivors.
+#include <cuda_fp16.h>
 #include "common.cuh"
 
 int sb_nms_launch(const float* boxes0, const float* boxes1, int stride, int n, float thresh,
@@ -333,6 +334,32 @@ rpn_head_epilogue_kernel(const float* __restrict__ head, long long total_pix, in
     for (int i = 0; i < 18; ++i) bp[i] = h[6 + i];
 }
 
+// stereo_rpn.py:89,116-119: the raw class scores the RPN loss reads, each pixel's six channels as three consecutive
+// pairs (c0,c1), (c2,c3), (c4,c5) -> rpn_cls_score [A,2]
+__global__ void __launch_bounds__(256)
+rpn_head_scores_kernel(const float* __restrict__ head, long long total_pix, int ld, float* __restrict__ score) {
+    const long long e = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (e >= total_pix * 6) return;
+    const long long p = e / 6;
+    score[e] = head[p * ld + (e - p * 6)];
+}
+
+// backward of the fused head's outputs: dhead[p][0..5] = s * d_cls[p*6 ..], dhead[p][6..23] = s * d_box[p*18 ..],
+// columns 24..63 zero (K padding of the head's data gradient and Cout padding of its weight gradient)
+__global__ void __launch_bounds__(256)
+rpn_head_grad_kernel(const float* __restrict__ d_cls, const float* __restrict__ d_box, long long total_pix,
+                     float grad_scale, __half* __restrict__ dhead16, float* __restrict__ dhead32) {
+    const long long e = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (e >= total_pix * 64) return;
+    const long long p = e >> 6;
+    const int c = (int)(e & 63);
+    float v = 0.f;
+    if (c < 6) v = grad_scale * __ldg(d_cls + p * 6 + c);
+    else if (c < 24) v = grad_scale * __ldg(d_box + p * 18 + (c - 6));
+    dhead16[e] = __float2half_rn(v);
+    if (dhead32) dhead32[e] = v;
+}
+
 struct WsLayout {
     size_t state, hist, block_eq, block_gt, cand, order, score, prop_l, prop_r, mask0, mask1, keep, num, total;
 };
@@ -481,6 +508,29 @@ extern "C" int sb_rpn_head_epilogue(const float* head, int B, int P, int ld, flo
     long long total = (long long)B * P;
     if (total <= 0) return total == 0 ? SB_OK : SB_EINVAL;
     rpn_head_epilogue_kernel<<<sb_div_up(total, 256), 256, 0, sb_cs(stream)>>>(head, total, ld, cls_prob, bbox_pred);
+    SB_LAUNCHED();
+    SB_CHECK_LAUNCH();
+    return SB_OK;
+}
+
+extern "C" int sb_rpn_head_scores(const float* head, int B, int P, int ld, float* rpn_cls_score, sb_stream_t stream) {
+    const long long total = (long long)B * P;
+    if (B < 0 || P < 0 || ld < 6 || (total > 0 && (!head || !rpn_cls_score))) return SB_EINVAL;
+    if (total == 0) return SB_OK;
+    rpn_head_scores_kernel<<<sb_div_up(total * 6, 256), 256, 0, sb_cs(stream)>>>(head, total, ld, rpn_cls_score);
+    SB_LAUNCHED();
+    SB_CHECK_LAUNCH();
+    return SB_OK;
+}
+
+extern "C" int sb_rpn_head_grad(const float* d_cls_score, const float* d_bbox_pred, int B, int P, float grad_scale,
+                                void* dhead16, float* dhead32, sb_stream_t stream) {
+    const long long total = (long long)B * P;
+    if (B < 0 || P < 0 || (total > 0 && (!d_cls_score || !d_bbox_pred || !dhead16))) return SB_EINVAL;
+    if ((reinterpret_cast<uintptr_t>(dhead16) & 1) || (reinterpret_cast<uintptr_t>(dhead32) & 3)) return SB_EINVAL;
+    if (total == 0) return SB_OK;
+    rpn_head_grad_kernel<<<sb_div_up(total * 64, 256), 256, 0, sb_cs(stream)>>>(
+        d_cls_score, d_bbox_pred, total, grad_scale, reinterpret_cast<__half*>(dhead16), dhead32);
     SB_LAUNCHED();
     SB_CHECK_LAUNCH();
     return SB_OK;

@@ -46,6 +46,29 @@ def trainable_trunk_fpn_params(fixed_blocks=1):
     return out
 
 
+def trainable_rpn_params():
+    """[(name, shape)] of the stereo RPN's parameters (stereo_rpn.py:32-39 of the reference), all trainable: RPN_Conv
+    (3x3, 256 -> 512, shared by both images and all five levels) and the two 1x1 heads on the 1024-channel
+    concatenation"""
+    return [("RCNN_rpn.RPN_Conv.weight", (512, 256, 3, 3)), ("RCNN_rpn.RPN_Conv.bias", (512,)),
+            ("RCNN_rpn.RPN_cls_score.weight", (6, 1024, 1, 1)), ("RCNN_rpn.RPN_cls_score.bias", (6,)),
+            ("RCNN_rpn.RPN_bbox_pred_left_right.weight", (18, 1024, 1, 1)),
+            ("RCNN_rpn.RPN_bbox_pred_left_right.bias", (18,))]
+
+
+class RpnSaved(object):
+    """what StereoRCNNEngine.rpn(save_for_backward=True) keeps for rpn_backward: per level the fp16 `cat` buffer
+    [B,h,w,1024] (the ReLU'd RPN_Conv outputs of L | R: the heads' input and the ReLU mask) and the fp16 P level
+    [2B,h,w,256] it read, plus the raw fused head output [B,P,32]"""
+    __slots__ = ("B", "shapes", "offs", "cats", "levels", "head")
+
+    def __init__(self, B, shapes, offs, cats, levels, head):
+        self.B, self.shapes, self.offs, self.cats, self.levels, self.head = B, shapes, offs, cats, levels, head
+
+
+_LEVELS = ("p2", "p3", "p4", "p5", "p6")
+
+
 # which lateral conv reads the input of RCNN_layer<li+1> (li = 1..3): c2 -> latlayer3, c3 -> latlayer2, c4 -> latlayer1
 _LATERAL_OF_INPUT = {1: ("RCNN_latlayer3", "dt2"), 2: ("RCNN_latlayer2", "dt3"), 3: ("RCNN_latlayer1", "dt4")}
 
@@ -129,8 +152,7 @@ class StereoRCNNEngine(object):
 
         def conv_bias(ck, pad):
             self.p[ck] = PackedConv(sd[ck + ".weight"], None, sd[ck + ".bias"].contiguous(), pad)
-            if not ck.startswith("RCNN_rpn"):
-                self._bwd_src[ck] = (sd[ck + ".weight"], None, pad)
+            self._bwd_src[ck] = (sd[ck + ".weight"], None, pad)
 
         # stem: [64,3,7,7] -> [64][7][7][3]
         s, b = bn_fold("RCNN_layer0.1")
@@ -159,6 +181,9 @@ class StereoRCNNEngine(object):
         bh[0:6] = sd["RCNN_rpn.RPN_cls_score.bias"]
         bh[6:24] = sd["RCNN_rpn.RPN_bbox_pred_left_right.bias"]
         self.p["rpn_heads"] = PackedConv(wh, None, bh, 0)
+        wh64 = torch.zeros(64, 1024, 1, 1)        # the head's data gradient: K = 64 rows (rows 24..63 zero)
+        wh64[:32] = wh
+        self._bwd_src["rpn_heads"] = (wh64, None, 0)
         # box head: Conv2d(512,2048,k=7,s=7) on a 7x7 map == FC over (ph,pw,c) of the NHWC pooled tile
         w0 = sd["RCNN_top.0.weight"]                                   # [2048,512,7,7]
         self.p["RCNN_top.0"] = PackedConv(_pack_conv(w0).reshape(2048, 7 * 7 * 512, 1, 1), None,
@@ -350,8 +375,9 @@ class StereoRCNNEngine(object):
 
     @property
     def found_inf(self):
-        """int32 [1] device flag: 1 when the last trunk_fpn_backward produced a non-finite gradient (cleared at the
-        start of every backward, never read on the host here -- torch.cuda.amp.GradScaler's found_inf)"""
+        """int32 [1] device flag: 1 when the last backward (rpn_backward, trunk_fpn_backward) produced a non-finite
+        gradient (cleared at the start of every backward unless it is told to keep it, never read on the host here --
+        torch.cuda.amp.GradScaler's found_inf)"""
         self._pack_backward()
         return self._found_inf[:1]
 
@@ -376,24 +402,30 @@ class StereoRCNNEngine(object):
                        grad_scale=gs, dy32=dy32, db=grads[key + ".bias"] if dy32 is not None else None,
                        nonfinite=self._found_inf)
 
-    def trunk_fpn_backward(self, saved, d_feats, fixed_blocks=1, grads=None, grad_scale=1.0):
+    def _grad_buffers(self, params, grads):
+        out = {}
+        for name, shape in params:
+            g = grads.get(name) if grads is not None else None
+            if g is None:
+                g = torch.empty(shape, dtype=torch.float32, device=self.device)
+            assert tuple(g.shape) == tuple(shape) and g.dtype == torch.float32 and g.is_contiguous(), name
+            out[name] = g
+        return out
+
+    def trunk_fpn_backward(self, saved, d_feats, fixed_blocks=1, grads=None, grad_scale=1.0, clear_found_inf=True):
         """Backward of trunk_fpn (ResNet-101 layers 1-4 + FPN, frozen BN) for the gradients d_feats["p2".."p6"] (fp32
         NHWC, the shapes trunk_fpn returns; left and right images batched, so every weight gradient sums over both).
         Returns {state_dict name: fp32 gradient} of exactly trainable_trunk_fpn_params(fixed_blocks), in the
         reference's layout; tensors given in `grads` (e.g. GradientBuckets views) are written in place.
         grad_scale (a power of two) multiplies dP before the fp16 chain and is divided out of the results exactly;
-        found_inf is set when a result is not finite.  No host synchronisation: graph-capturable."""
+        found_inf is set when a result is not finite; clear_found_inf=False keeps a flag an earlier backward of the
+        same step set (rpn_backward before this).  No host synchronisation: graph-capturable."""
         self._pack_backward()
         dev = self.device
         gs = float(grad_scale)
-        out = {}
-        for name, shape in trainable_trunk_fpn_params(fixed_blocks):
-            g = grads.get(name) if grads is not None else None
-            if g is None:
-                g = torch.empty(shape, dtype=torch.float32, device=dev)
-            assert tuple(g.shape) == tuple(shape) and g.dtype == torch.float32 and g.is_contiguous(), name
-            out[name] = g
-        ops.fill_(self._found_inf, 0.0)
+        out = self._grad_buffers(trainable_trunk_fpn_params(fixed_blocks), grads)
+        if clear_found_inf:
+            ops.fill_(self._found_inf, 0.0)
         dp = {k: ops._f32c(d_feats[k]) for k in ("p2", "p3", "p4", "p5", "p6")}
         # ---- FPN (stereo_rcnn.py:155-168): P2 <- smooth3(lat3(c2) + up(P3)) ... P5 = toplayer(c5), P6 = P5[::2, ::2]
         g32, g16 = ops.fpn_grad_combine(dp["p2"], scale=gs)
@@ -439,16 +471,28 @@ class StereoRCNNEngine(object):
                 g32, g16 = self._dgrad(dt[dtk], lat, residual=scat, mask=xf)
         return out
 
-    def rpn(self, feats, B):
-        """stereo_rpn.py:73-95 -> cls_prob [B,A,2], bbox_pred [B,A,6], level shapes"""
+    def rpn(self, feats, B, save_for_backward=False):
+        """stereo_rpn.py:73-95 -> cls_prob [B,A,2], bbox_pred [B,A,6], level shapes.
+        save_for_backward=True (fp16-operand engines) also returns an RpnSaved for rpn_backward and the raw class
+        scores rpn_cls_score [B,A,2] the RPN loss reads; cls_prob and bbox_pred are the same bits either way."""
+        if save_for_backward and not self.half:
+            raise ValueError("the backward pass runs on fp16 conv operands: build the engine with precision='fp16'")
         sfx = "_16" if self.half else ""
         levels = [feats[k + sfx] for k in ("p2", "p3", "p4", "p5", "p6")]
         shapes = [[f.shape[1], f.shape[2]] for f in levels]
         P = sum(h * w for h, w in shapes)
         dev = self.device
         head = torch.empty(B, P, 32, dtype=torch.float32, device=dev)
-        def level(f, h, w, off):
-            cat = torch.empty(B, h, w, 1024, dtype=f.dtype, device=dev)
+        offs = [0]
+        for h, w in shapes:
+            offs.append(offs[-1] + h * w)
+        # saved for the backward: allocated here on the current stream, not inside the side-stream fork below
+        cats = ([torch.empty(B, h, w, 1024, dtype=torch.float16, device=dev) for h, w in shapes]
+                if save_for_backward else [None] * len(shapes))
+
+        def level(f, h, w, off, cat=None):
+            if cat is None:
+                cat = torch.empty(B, h, w, 1024, dtype=f.dtype, device=dev)
             kw = dict(f32=False, out16=cat) if self.half else dict(out=cat, out_mode=ops.ROUND_TF32)
             if B == 1:      # L and R in one launch: image index n = side -> channel offset n * 512
                 self._conv(f, self.p["RCNN_rpn.RPN_Conv"], relu=True, out_strides=(512, w * 1024, 1024),
@@ -459,22 +503,72 @@ class StereoRCNNEngine(object):
                                out_coff=side * 512, out_strides=(h * w * 1024, w * 1024, 1024), tag="rpn_conv", **kw)
             self._conv(cat, self.p["rpn_heads"], out=head[:, off:off + h * w],
                        out_strides=(P * 32, w * 32, 32), tag="rpn_heads")
-        offs = [0]
-        for h, w in shapes:
-            offs.append(offs[-1] + h * w)
         fork = self.side is not None and self.forks
         if fork:    # the three coarse levels are a handful of tiles each: run them beside the p2 / p3 convs
             main = torch.cuda.current_stream()
             self.side.wait_stream(main)
             with torch.cuda.stream(self.side):
                 for i in (2, 3, 4):
-                    level(levels[i], shapes[i][0], shapes[i][1], offs[i])
+                    level(levels[i], shapes[i][0], shapes[i][1], offs[i], cats[i])
         for i in ((0, 1) if fork else range(5)):
-            level(levels[i], shapes[i][0], shapes[i][1], offs[i])
+            level(levels[i], shapes[i][0], shapes[i][1], offs[i], cats[i])
         if fork:
             main.wait_stream(self.side)
         cls_prob, bbox = ops.rpn_head_epilogue(head, B, P)
+        if save_for_backward:
+            return (cls_prob, bbox, shapes, RpnSaved(B, shapes, offs, cats, levels, head),
+                    ops.rpn_head_scores(head, B, P))
         return cls_prob, bbox, shapes
+
+    def rpn_backward(self, saved, d_cls_score, d_bbox_pred, grads=None, grad_scale=1.0):
+        """Backward of rpn (stereo_rpn.py:73-95) for the RPN loss gradients d_cls_score [B,A,2] (w.r.t. the raw scores
+        rpn returns) and d_bbox_pred [B,A,6].  Returns ({state_dict name: fp32 gradient} of exactly
+        trainable_rpn_params(), in the reference's layout; tensors given in `grads` are written in place,
+        {"p2".."p6": dP fp32 [2B,h,w,256]} for trunk_fpn_backward).  Weight gradients are summed over the levels
+        P2..P6 and, for RPN_Conv, left before right: a fixed order, bit-identical run to run.  grad_scale (a power of
+        two) scales the fp16 chain and is divided out of every result exactly; found_inf is cleared, then set when a
+        gradient is not finite.  No host synchronisation: graph-capturable."""
+        self._pack_backward()
+        dev = self.device
+        gs = float(grad_scale)
+        B, offs = saved.B, saved.offs
+        P = offs[-1]
+        out = self._grad_buffers(trainable_rpn_params(), grads)
+        ops.fill_(self._found_inf, 0.0)
+        dh16, dh32 = ops.rpn_head_grad(d_cls_score, d_bbox_pred, B, P, gs)
+        # the dgrad epilogue's per-channel scale divides grad_scale out of dP (exact: a power of two)
+        unscale = ops.fill_(torch.empty(256, dtype=torch.float32, device=dev), 1.0 / gs) if gs != 1.0 else None
+        hd, cd = self._bwd["rpn_heads"], self._bwd["RCNN_rpn.RPN_Conv"]
+        w_cls, w_box = out["RCNN_rpn.RPN_cls_score.weight"], out["RCNN_rpn.RPN_bbox_pred_left_right.weight"]
+        b_cls, b_box = out["RCNN_rpn.RPN_cls_score.bias"], out["RCNN_rpn.RPN_bbox_pred_left_right.bias"]
+        w_conv, b_conv = out["RCNN_rpn.RPN_Conv.weight"], out["RCNN_rpn.RPN_Conv.bias"]
+        dps = {}
+        for i, (h, w) in enumerate(saved.shapes):
+            cat, f16 = saved.cats[i], saved.levels[i]
+            dcat32 = torch.empty(B, h, w, 1024, dtype=torch.float32, device=dev)
+            dcat16 = torch.empty(B, h, w, 1024, dtype=torch.float16, device=dev)
+            for b in range(B):
+                # fused 1x1 head: dW / db rows 0..5 -> RPN_cls_score, 6..23 -> RPN_bbox_pred_left_right
+                dy16 = dh16[b, offs[i]:offs[i + 1]].view(1, h, w, 64)
+                dy32 = dh32[b, offs[i]:offs[i + 1]].view(1, h, w, 64)
+                ops.conv_wgrad_acc(dy16, cat[b:b + 1], 1, w_cls, db=b_cls, dy32=dy32, grad_scale=gs,
+                                   accumulate=i > 0 or b > 0, rows=24, split=6, dw_hi=w_box, db_hi=b_box,
+                                   nonfinite=self._found_inf)
+                # d cat = head^T dhead where cat > 0 (the ReLU of RPN_Conv; cat has the output's layout)
+                d = ops.conv_desc(dy16, hd.w16, dcat32[b:b + 1], hd.Cin, hd.Cout, 1, 1, 1, 0, h, w,
+                                  out16=dcat16[b:b + 1])
+                ops.conv2d_dgrad(d, cat[b:b + 1])
+            dp = torch.empty(2 * B, h, w, 256, dtype=torch.float32, device=dev)
+            for side in range(2):       # RPN_Conv on L then R: channel halves 0..511 and 512..1023 of d cat
+                c0 = side * 512
+                ops.conv_wgrad_acc(dcat16[..., c0:c0 + 512], f16[side * B:(side + 1) * B], 3, w_conv, db=b_conv,
+                                   dy32=dcat32[..., c0:c0 + 512], grad_scale=gs, accumulate=i > 0 or side > 0,
+                                   nonfinite=self._found_inf)
+                d = ops.conv_desc(dcat16[..., c0:c0 + 512], cd.w16, dp[side * B:(side + 1) * B], cd.Cin, cd.Cout, 3, 3, 1, 1,
+                                  h, w, scale=unscale, in_ld=1024)
+                ops.conv2d_dgrad(d)
+            dps[_LEVELS[i]] = dp
+        return out, dps
 
     def heads(self, feats, B, rois_l, rois_r, im_h):
         """stereo_rcnn.py:240-271 on flattened rois [R,5]"""

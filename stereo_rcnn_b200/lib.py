@@ -64,6 +64,7 @@ _SIGS = {
                                   c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "sb_generate_anchors": (c_int, [ctypes.POINTER(ProposalCfg), c_int, c_void_p, c_void_p]),
     "sb_rpn_head_epilogue": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "sb_rpn_head_scores": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "sb_dense_align_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "sb_dense_align": (c_int, [c_void_p, c_void_p, c_int, c_int, ctypes.POINTER(c_double), c_double,
                                c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t,
@@ -85,6 +86,10 @@ _SIGS = {
                       [c_void_p, c_size_t, c_void_p]),
     "sb_fpn_grad_combine": (c_int, [c_void_p, c_void_p] + [c_int] * 6 + [c_void_p, c_int, c_int, c_float, c_void_p,
                                     c_void_p, c_void_p]),
+    "sb_rpn_head_grad": (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]),
+    "sb_conv_wgrad_acc_workspace": (c_size_t, [c_int] * 6),
+    "sb_conv_wgrad_acc": (c_int, [c_void_p, c_int, c_void_p] + [c_int] * 7 + [c_void_p, c_float, c_void_p] +
+                          [c_int] * 4 + [c_void_p] * 6 + [c_size_t, c_void_p]),
     "sb_conv_trace_bytes": (c_size_t, [c_int]),
     "sb_conv_trace": (c_int, [c_void_p, c_int]),
     "sb_conv_trace_count": (c_int, []),

@@ -325,9 +325,10 @@ def kitti_result_lines(final, t_cam2_cam0_x):
 # ------------------------------------------------------------- layer ops ----
 def conv_desc(x, wgt, out, Cin, Cout, kh, kw, stride, pad, Ho, Wo, scale=None, shift=None, residual=None,
               up_src=None, relu=False, out_coff=0, out_strides=None, out_mode=0, res_biased=False,
-              in_biased=False, out16=None, max_ctas=0):
+              in_biased=False, out16=None, max_ctas=0, in_ld=None):
     """x: NHWC [N,H,W,in_ld]; wgt packed [Cout,kh,kw,Cin]; out: any tensor addressed through out_strides
-    = (n, h, w) strides in floats (default: dense NHWC of out.shape[-1] channels)."""
+    = (n, h, w) strides in floats (default: dense NHWC of out.shape[-1] channels).  in_ld: pixel stride of x in
+    elements (default x.shape[3]; a channel slice of a wider tensor passes the wider tensor's)."""
     d = ConvDesc()
     N, H, W = x.shape[0], x.shape[1], x.shape[2]
     d.in_, d.wgt = x.data_ptr(), wgt.data_ptr()
@@ -342,7 +343,7 @@ def conv_desc(x, wgt, out, Cin, Cout, kh, kw, stride, pad, Ho, Wo, scale=None, s
     d.up_src = up_src.data_ptr() if up_src is not None else None
     d.N, d.H, d.W, d.Cin, d.Cout, d.kh, d.kw = N, H, W, Cin, Cout, kh, kw
     d.stride, d.pad, d.Ho, d.Wo = stride, pad, Ho, Wo
-    d.in_ld = x.shape[3]
+    d.in_ld = x.shape[3] if in_ld is None else int(in_ld)
     d.res_ld = _flat_rows_ld(residual) if residual is not None else 0
     d.UH, d.UW = (up_src.shape[1], up_src.shape[2]) if up_src is not None else (0, 0)
     d.relu = 1 if relu else 0
@@ -404,6 +405,63 @@ def conv_wgrad(dy16, x16, k, dw, scale=None, grad_scale=1.0, dy32=None, db=None,
     check(L.sb_conv_wgrad(ptr(dy16), ptr(x16), N, H, W, Cin, Cout, k, ptr(scale), float(1.0 / grad_scale), ptr(dw),
                           ptr(dy32), ptr(db), ptr(nonfinite), ptr(ws), nb, stream_ptr()), "sb_conv_wgrad")
     return dw, db
+
+
+def _vptr(t):
+    """device pointer of a CUDA tensor that may be a strided view (None -> NULL)"""
+    if t is None:
+        return ctypes.c_void_p(0)
+    assert t.is_cuda
+    return ctypes.c_void_p(t.data_ptr())
+
+
+def conv_wgrad_acc(dy16, x16, k, dw, db=None, dy32=None, scale=None, grad_scale=1.0, accumulate=False, rows=None,
+                   split=None, dw_hi=None, db_hi=None, nonfinite=None):
+    """conv_wgrad on NHWC views whose pixels are rows of one pitch (dy16 may be a channel slice of a wider tensor),
+    optionally added to dw / db (accumulate=True).  Rows [0, split) of dW / db go to dw / db, rows [split, rows) to
+    dw_hi / db_hi, rows past `rows` are dropped (defaults: rows = split = Cout)."""
+    L = _l.load()
+    N, H, W, Cout = dy16.shape
+    Cin = x16.shape[3]
+    assert dy16.dtype == torch.float16 and x16.dtype == torch.float16 and tuple(x16.shape[:3]) == (N, H, W)
+    rows = Cout if rows is None else int(rows)
+    split = rows if split is None else int(split)
+    kk = Cin * k * k
+    assert dw.dtype == torch.float32 and dw.is_contiguous() and dw.numel() == split * kk
+    assert dw_hi is None or (dw_hi.dtype == torch.float32 and dw_hi.is_contiguous() and
+                             dw_hi.numel() == (rows - split) * kk)
+    for b, n in ((db, split), (db_hi, rows - split)):
+        assert b is None or (b.dtype == torch.float32 and b.is_contiguous() and b.numel() == n)
+    assert dy32 is None or (dy32.dtype == torch.float32 and tuple(dy32.shape) == (N, H, W, Cout))
+    nb = L.sb_conv_wgrad_acc_workspace(N, H, W, Cin, Cout, k)
+    ws = workspace(nb, dy16.device, "wgrad")
+    check(L.sb_conv_wgrad_acc(_vptr(dy16), _flat_rows_ld(dy16), _vptr(x16), _flat_rows_ld(x16), N, H, W, Cin, Cout, k,
+                              ptr(scale), float(1.0 / grad_scale), _vptr(dy32),
+                              _flat_rows_ld(dy32) if dy32 is not None else 0, int(bool(accumulate)), rows, split,
+                              ptr(dw), ptr(db), ptr(dw_hi), ptr(db_hi), ptr(nonfinite), ptr(ws), nb, stream_ptr()),
+          "sb_conv_wgrad_acc")
+    return dw, db
+
+
+def rpn_head_scores(head, B, P):
+    """raw fused head output [B, P, ld] -> the loss's raw class scores rpn_cls_score [B, 3P, 2]"""
+    L = _l.load()
+    score = torch.empty(B, 3 * P, 2, dtype=torch.float32, device=head.device)
+    check(L.sb_rpn_head_scores(ptr(head), B, P, head.shape[-1], ptr(score), stream_ptr()), "sb_rpn_head_scores")
+    return score
+
+
+def rpn_head_grad(d_cls_score, d_bbox_pred, B, P, grad_scale=1.0, f32=True):
+    """d rpn_cls_score [B,3P,2], d rpn_bbox_pred [B,3P,6] -> (dhead16 [B,P,64] fp16, dhead32 [B,P,64] fp32 or None):
+    grad_scale * d in the fused head's rows 0..23, zero in 24..63"""
+    L = _l.load()
+    assert tuple(d_cls_score.shape) == (B, 3 * P, 2) and tuple(d_bbox_pred.shape) == (B, 3 * P, 6)
+    dev = d_cls_score.device
+    dh16 = torch.empty(B, P, 64, dtype=torch.float16, device=dev)
+    dh32 = torch.empty(B, P, 64, dtype=torch.float32, device=dev) if f32 else None
+    check(L.sb_rpn_head_grad(ptr(_f32c(d_cls_score)), ptr(_f32c(d_bbox_pred)), B, P, float(grad_scale), ptr(dh16),
+                             ptr(dh32), stream_ptr()), "sb_rpn_head_grad")
+    return dh16, dh32
 
 
 def fpn_grad_combine(dp=None, dt=None, dp6=None, scale=1.0, shape=None, out=None, out16=None, f32=True, f16=True):

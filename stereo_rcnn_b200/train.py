@@ -4,7 +4,8 @@ Host-side mirror of `_AnchorTargetLayer` (lib/model/rpn/anchor_target_layer.py:4
 (lib/model/rpn/proposal_target_layer.py:36-333), the RPN / RCNN losses (stereo_rpn.py:114-140,
 stereo_rcnn.py:201-311), the multi-task sum (trainval_net.py:214-219) and `clip_gradient` (net_utils.py:37-49) over
 libstereo_b200's kernels (csrc/train_targets.cu, csrc/train_loss.cu).  No host synchronisation anywhere: counts,
-sampled indices and losses stay on the device.  Backbone dgrad / wgrad is NOT part of this module.
+sampled indices and losses stay on the device.  rpn_gradients composes them with the engine's forward and backward
+passes into the gradients of the RPN loss for the trunk, the FPN and the RPN.
 """
 import ctypes
 
@@ -173,3 +174,32 @@ def clip_gradient(grads, clip_norm):
     check(L.sb_clip_gradient(ptrs, counts, n, float(clip_norm), ptr(ws), nbytes, ptr(out), stream_ptr()),
           "sb_clip_gradient")
     return out
+
+
+def rpn_gradients(engine, im_left, im_right, gt_left, gt_right, gt_merge, keys, uncert=None, fixed_blocks=1,
+                  grads=None, grad_scale=1.0):
+    """The RPN loss of a stereo pair differentiated end to end on the device (stereo_rpn.py:114-140 through
+    stereo_rpn.py:73-95 and the trunk + FPN): trunk_fpn and rpn with save_for_backward, the anchor targets for
+    `keys` (anchor_targets), rpn_loss, then rpn_backward and trunk_fpn_backward(fixed_blocks).
+    im_left / im_right [B,3,H,W] NCHW fp32 network inputs, gt_* [B,K,5], keys [B,A] int32 words.
+    Returns (losses [2] = (rpn_loss_cls, rpn_loss_box), {state_dict name: fp32 gradient} of
+    trainable_trunk_fpn_params(fixed_blocks) + trainable_rpn_params()) and, with uncert [>= 2] (the multi-task
+    weights of trainval_net.py:214-219), d total / d uncert[0:2] as a third item; the gradients are then those of
+    losses[i] * exp(-uncert[i]).  grads / grad_scale as in rpn_backward; engine.found_inf covers both backward
+    passes.  No optimizer step, no host synchronisation."""
+    B, _, H, W = im_left.shape
+    with torch.no_grad():
+        im = torch.cat((im_left, im_right), 0).contiguous()
+        feats, saved_t = engine.trunk_fpn(im, save_for_backward=True)
+        _cls_prob, bbox, shapes, saved_r, score = engine.rpn(feats, B, save_for_backward=True)
+        anchors = generate_anchors(shapes, im.device)
+        labels, tl, tr, iw, ow = anchor_targets(anchors, gt_left, gt_right, gt_merge, (H, W), keys)
+        u = uncert[0:2] if uncert is not None else None
+        losses, d_cls, d_box = rpn_loss(score, bbox, labels, tl, tr, iw, ow, uncert=u)
+        g, dp = engine.rpn_backward(saved_r, d_cls, d_box, grads=grads, grad_scale=grad_scale)
+        g.update(engine.trunk_fpn_backward(saved_t, dp, fixed_blocks=fixed_blocks, grads=grads, grad_scale=grad_scale,
+                                           clear_found_inf=False))
+        if uncert is None:
+            return losses, g
+        _total, d_u = multitask_loss(losses, u)
+        return losses, g, d_u
