@@ -470,7 +470,7 @@ def fpn_grad_combine(dp=None, dt=None, dp6=None, scale=1.0, shape=None, out=None
     P6 = P5[::2, ::2].  shape = (N, H, W, C) when dp is None.  Returns (fp32, fp16) as requested."""
     L = _l.load()
     N, H, W, C = dp.shape if dp is not None else shape
-    dev = (dp if dp is not None else dt).device
+    dev = next(t.device for t in (dp, dt, dp6) if t is not None)
     if out is None and f32:
         out = torch.empty(N, H, W, C, dtype=torch.float32, device=dev)
     if out16 is None and f16:
