@@ -177,6 +177,11 @@ int sb_conv2d_simt(const sb_conv_desc* d, sb_stream_t stream);
  * pixel strides), and with a twin Cout, out_w_stride and out_coff % 8 == 0 and out16 16-byte aligned. */
 int sb_conv2d_tc(const sb_conv_desc* d, sb_stream_t stream);
 int sb_conv2d_tc_supported(const sb_conv_desc* d);
+/* the same 3x3 convolution on flat tiles of 128 consecutive output pixels in (n, h, w) order, loaded by TMA im2col,
+ * instead of 8x16 spatial patches: no MMA rows past the right or bottom edge of a map.  Bit-identical to sb_conv2d_tc
+ * on the descriptors it takes: what sb_conv2d_tc_supported() accepts with fp16 operands, 3x3, pad 1, stride 1, no
+ * residual and no up_src; SB_EINVAL for anything else, before any launch. */
+int sb_conv2d_tc_rows(const sb_conv_desc* d, sb_stream_t stream);
 
 /* ------------------------------------------------- backward pass of the trunk + FPN (fp16 operands, fp32 accumulate) ----
  * sb_conv2d_tc_dgrad -- data gradient of a conv (the input gradient torch.nn.Conv2d's autograd forms for the convs of

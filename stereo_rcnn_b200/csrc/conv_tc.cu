@@ -15,6 +15,9 @@
 //     of a flat [M, Cin] matrix) or a 4-D [C, W, H, N] map (3x3: an 8x16 pixel patch per tile; the tap shift is a
 //     coordinate offset and the hardware zero-fills the padding halo, so im2col never exists in memory).  128-byte
 //     swizzle, 1024-byte aligned stages, one 128-byte row (64 fp16 / 32 fp32 = one K-step) per pixel per stage.
+//     sb_conv2d_tc_rows runs fp16 3x3 convs on flat tiles of 128 consecutive output pixels instead: a TMA im2col map
+//     loads them shifted by the tap (zero-filled halo at every row and image edge, inside a tile too), so no MMA row
+//     is spent on pixels past the edge of a map; the shared-memory tile is that of a 1x1 conv's flat rows.
 //     The stem variant builds its A tile in the kernel instead (patch gather warps, see below).
 //   * warp-specialised persistent CTAs (one per SM): warps 0..7 are two consumer warpgroups -- each issues the
 //     m64nNk16 (k8 for tf32) wgmma of 64 of the tile's 128 rows and owns their fp32 accumulators -- and warp 8 is
@@ -64,6 +67,7 @@ struct TcParams {
     int num_m_tiles, num_n_tiles;
     int kblocks_per_tap;  // Cin / BLOCK_K
     int num_k_blocks;     // taps * kblocks_per_tap
+    int rows;             // 1 (patch 0): 3x3 / pad 1 on flat rows of 128 output pixels, A by TMA im2col
     long long M;
     unsigned long long* trace;   // optional per-CTA phase timestamps (sb_conv_trace), 16 words per CTA
     // STEM variant: the A operand is gathered from the NCHW fp32 image [N,3,sH,sW] (7x7 / stride 2 / pad 3 patches)
@@ -167,6 +171,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                     h0 = (t2 % p.tiles_h) * TH;
                     n_img = t2 / p.tiles_h;
                     w0 = tw * TW;
+                } else if (!STEM && p.rows) {      // the tile's first output pixel
+                    const unsigned m0 = (unsigned)mt * BLOCK_M, hw = (unsigned)(d.Ho * d.Wo);
+                    n_img = (int)(m0 / hw);
+                    const unsigned rem = m0 - (unsigned)n_img * hw;
+                    h0 = (int)(rem / (unsigned)d.Wo);
+                    w0 = (int)(rem - (unsigned)h0 * (unsigned)d.Wo);
                 }
                 for (int kb = 0; kb < p.num_k_blocks; ++kb) {
                     const int tap = kb / p.kblocks_per_tap;
@@ -178,6 +188,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                         if (p.patch) {
                             const int r = tap / d.kw, s = tap - r * d.kw;
                             tma_load_4d(&map_a, &full[stage], sa, c0, w0 + s - d.pad, h0 + r - d.pad, n_img);
+                        } else if (p.rows) {
+                            // the bounding box holds the taps' origins (output pixel - pad); each tap is an offset
+                            const int r = tap / d.kw, s = tap - r * d.kw;
+                            tma_load_im2col_4d(&map_a, &full[stage], sa, c0, w0 - d.pad, h0 - d.pad, n_img,
+                                               (uint16_t)s, (uint16_t)r);
                         } else {
                             tma_load_2d(&map_a, &full[stage], sa, c0, mt * BLOCK_M);
                         }
@@ -519,6 +534,43 @@ bool make_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims
     return r == CUDA_SUCCESS;
 }
 
+typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                   const cuuint64_t*, const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*,
+                                   CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
+                                   CUtensorMapFloatOOBfill);
+
+EncodeIm2colFn get_encode_im2col() {
+    static EncodeIm2colFn fn = nullptr;
+    if (!fn) {
+        void* p = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &p, cudaEnableDefault, &qres) != cudaSuccess ||
+            qres != cudaDriverEntryPointSuccess)
+            return nullptr;
+        fn = (EncodeIm2colFn)p;
+    }
+    return fn;
+}
+
+// im2col map of a 3x3 / pad 1 / stride 1 conv over fp16 NHWC activations [N, H, W, in_ld] (channels [0, Cin) used):
+// a load brings the BLOCK_M pixels that follow its start coordinate in (n, h, w) order, 64 channels (128 bytes) each,
+// 128-byte swizzled -- the layout of the flat 2-D [M, Cin] box of a 1x1 conv.  The bounding box holds the origins of
+// the taps, output pixel - pad: w in [-1, W - 2] (lower corner -1, upper corner W - 1 + (-1)), h alike; the tap
+// offsets (s, r) in 0..2 shift every pixel, and what lands outside [0, W) x [0, H) is zero-filled.
+bool make_map_im2col3x3(CUtensorMap* m, const sb_conv_desc* d) {
+    EncodeIm2colFn enc = get_encode_im2col();
+    if (!enc) return false;
+    const cuuint64_t dims[4] = {(cuuint64_t)d->Cin, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->N};
+    const cuuint64_t strides[3] = {(cuuint64_t)d->in_ld * 2, (cuuint64_t)d->W * d->in_ld * 2,
+                                   (cuuint64_t)d->H * d->W * d->in_ld * 2};
+    const int lower[2] = {-d->pad, -d->pad}, upper[2] = {d->pad - (d->kw - 1), d->pad - (d->kh - 1)};
+    const cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(static_cast<const void*>(d->in)), dims,
+                     strides, lower, upper, 64, BLOCK_M, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return r == CUDA_SUCCESS;
+}
+
 // Tile-width choice.  Per SM and clock an H100 retires ~1024 dense fp16 MACs and ingests ~64 B from L2, so a
 // 64-element K-step of a 128-row tile costs max(MMA cycles, bytes / 64):
 //   BN=128: max(1024 * 128 * 64 / 1024 / 8, (16+16) KB / 64) = 512 cycles    BN=256: max(1024, (16+32) KB / 64) = 1024
@@ -661,7 +713,9 @@ extern "C" int sb_conv_trace_info(int id, int* out12) {
 extern "C" int sb_conv_trace_count(void) { return g_trace_n; }
 
 namespace {
-int conv2d_tc(const sb_conv_desc* d, const __half* mask16, bool dgrad, sb_stream_t stream) {
+// rows: flat 128-pixel tiles loaded by TMA im2col for a 3x3 conv (sb_conv2d_tc_rows; the caller has checked the
+// descriptor)
+int conv2d_tc(const sb_conv_desc* d, const __half* mask16, bool dgrad, bool rows, sb_stream_t stream) {
     if (!supported(d, dgrad)) return SB_EINVAL;
     TcParams p;
     p.d = *d;
@@ -671,7 +725,8 @@ int conv2d_tc(const sb_conv_desc* d, const __half* mask16, bool dgrad, sb_stream
     p.sH = p.sW = 0;
     // spatial 8x16 tiles for 3x3 convs, and for the FPN laterals so that the bilinear upsample taps of a tile
     // (5x9 source pixels) stay in L1 instead of being re-fetched from L2 for every output row
-    p.patch = (d->kh == 3 || d->up_src) ? 1 : 0;
+    p.patch = !rows && (d->kh == 3 || d->up_src) ? 1 : 0;
+    p.rows = rows ? 1 : 0;
     p.M = (long long)d->N * d->Ho * d->Wo;
     if (p.M == 0) return SB_OK;
     const bool f16 = d->in_dtype == 1;
@@ -700,7 +755,9 @@ int conv2d_tc(const sb_conv_desc* d, const __half* mask16, bool dgrad, sb_stream
     TcMaps m;
     memset(&m, 0, sizeof(m));
     CUtensorMap &ma = m.a, &mb = m.b;
-    if (p.patch) {
+    if (p.rows) {
+        if (!make_map_im2col3x3(&ma, d)) return SB_EINVAL;
+    } else if (p.patch) {
         cuuint64_t dims[4] = {(cuuint64_t)d->Cin, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->N};
         cuuint64_t strides[3] = {(cuuint64_t)d->in_ld * esz, (cuuint64_t)d->W * d->in_ld * esz,
                                  (cuuint64_t)d->H * d->W * d->in_ld * esz};
@@ -742,7 +799,21 @@ int conv2d_tc(const sb_conv_desc* d, const __half* mask16, bool dgrad, sb_stream
 }
 }  // namespace
 
-extern "C" int sb_conv2d_tc(const sb_conv_desc* d, sb_stream_t stream) { return conv2d_tc(d, nullptr, false, stream); }
+extern "C" int sb_conv2d_tc(const sb_conv_desc* d, sb_stream_t stream) {
+    return conv2d_tc(d, nullptr, false, false, stream);
+}
+
+// A 3x3 conv on 8x16 patches issues all 128 MMA rows of a patch that runs past the right or bottom edge of its map
+// (a 14x14 map takes two patches, 256 rows for 196 pixels).  Flat tiles of 128 consecutive output pixels, loaded
+// by TMA im2col one tap at a time, issue only the rows of the last tile past M.  Per output pixel the A values and
+// the K order (tap-major, then Cin chunks) are those of the patch path, so the results are bit-identical to
+// sb_conv2d_tc's.  Same kernel instantiations, epilogue of the flat rows (any out strides).
+extern "C" int sb_conv2d_tc_rows(const sb_conv_desc* d, sb_stream_t stream) {
+    if (!d || d->in_dtype != 1 || d->kh != 3 || d->kw != 3 || d->pad != 1 || d->stride != 1 || d->residual ||
+        d->up_src)
+        return SB_EINVAL;
+    return conv2d_tc(d, nullptr, false, true, stream);
+}
 
 // Data gradient of a convolution as the forward implicit GEMM on transposed weights (the caller packs them
 // [Cin][kh][kw][Cout], taps flipped, frozen-BN scale folded in), with the ReLU mask of a saved tensor applied after
@@ -750,7 +821,7 @@ extern "C" int sb_conv2d_tc(const sb_conv_desc* d, sb_stream_t stream) { return 
 extern "C" int sb_conv2d_tc_dgrad(const sb_conv_desc* d, const void* mask16, sb_stream_t stream) {
     if (!d || d->in_dtype != 1 || d->up_src || d->relu || d->out_mode != 0) return SB_EINVAL;
     if (reinterpret_cast<uintptr_t>(mask16) & 3) return SB_EINVAL;
-    return conv2d_tc(d, reinterpret_cast<const __half*>(mask16), true, stream);
+    return conv2d_tc(d, reinterpret_cast<const __half*>(mask16), true, false, stream);
 }
 
 // The stem (resnet.py:111-112: Conv2d(3, 64, 7, stride 2, pad 3) + frozen BN + ReLU) as an implicit GEMM on the tensor

@@ -52,6 +52,19 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* map, uint64_t* ba
         "r"(c2), "r"(c3)
         : "memory");
 }
+// TMA im2col load of a 4-D [C, W, H, N] tensor (map from cuTensorMapEncodeIm2col): the map's pixelsPerColumn pixels
+// that follow (w, h, n) in (n, h, w) order inside the map's bounding box, each shifted by (off_w, off_h), c0.. of
+// their channels; elements outside the tensor (the padding halo, pixels past the last image) are zero-filled and
+// count toward complete_tx
+__device__ __forceinline__ void tma_load_im2col_4d(const CUtensorMap* map, uint64_t* bar, void* smem, int c0, int w,
+                                                   int h, int n, uint16_t off_w, uint16_t off_h) {
+    asm volatile(
+        "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes"
+        " [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
+        ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(w), "r"(h),
+        "r"(n), "h"(off_w), "h"(off_h)
+        : "memory");
+}
 // TMA store of a shared-memory box, tracked by the issuing thread's bulk async-group
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t saddr, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"

@@ -227,7 +227,14 @@ class StereoRCNNEngine(object):
                           pc.kw, stride, pc.pad, Ho, Wo, scale=pc.scale, shift=pc.shift, residual=residual,
                           up_src=up_src, relu=relu, out_coff=out_coff, out_strides=out_strides, out_mode=out_mode,
                           res_biased=res_biased, in_biased=in_biased, out16=out16)
-        impl = ops.conv2d(d, "tc" if half_in else self.conv_impl)
+        if half_in and pc.kh == 3 and stride == 1 and residual is None and up_src is None:
+            # fp16 3x3: flat 128-pixel tiles by TMA im2col, the same bits as the 8x16 patches of sb_conv2d_tc without
+            # their MMA rows past the map edges.  Recorded as "tc": bench.py's roofline re-launches the descriptor
+            # through sb_conv2d_tc, so it times these convs on patches.
+            ops.conv2d_rows(d)
+            impl = "tc"
+        else:
+            impl = ops.conv2d(d, "tc" if half_in else self.conv_impl)
         if self.record is not None:
             self.record.append((d, impl, (x, out, out16, residual, up_src)))
         if tag is not None:

@@ -80,6 +80,7 @@ _SIGS = {
     "sb_conv2d_simt": (c_int, [ctypes.POINTER(ConvDesc), c_void_p]),
     "sb_conv2d_tc": (c_int, [ctypes.POINTER(ConvDesc), c_void_p]),
     "sb_conv2d_tc_supported": (c_int, [ctypes.POINTER(ConvDesc)]),
+    "sb_conv2d_tc_rows": (c_int, [ctypes.POINTER(ConvDesc), c_void_p]),
     "sb_conv2d_tc_dgrad": (c_int, [ctypes.POINTER(ConvDesc), c_void_p, c_void_p]),
     "sb_conv_wgrad_workspace": (c_size_t, [c_int] * 6),
     "sb_conv_wgrad": (c_int, [c_void_p, c_void_p] + [c_int] * 6 + [c_void_p, c_float] + [c_void_p] * 4 +

@@ -384,6 +384,13 @@ def conv2d(desc, impl="auto"):
     return impl
 
 
+def conv2d_rows(desc):
+    """fp16 3x3 / pad 1 / stride 1 conv without residual or upsample source on flat 128-pixel tiles (TMA im2col):
+    bit-identical to conv2d(desc, "tc") with fewer MMA rows past the map edges; anything else raises"""
+    L = _l.load()
+    check(L.sb_conv2d_tc_rows(ctypes.byref(desc), stream_ptr()), "sb_conv2d_tc_rows")
+
+
 def conv2d_dgrad(desc, mask16=None):
     """data gradient through the tensor-core conv (desc built on transposed weights, see sb_conv2d_tc_dgrad);
     mask16: fp16 tensor with the output's layout whose ReLU mask (> 0) is applied after the residual add"""
