@@ -228,6 +228,50 @@ int sb_conv_wgrad_acc(const void* dy16, int dy_ld, const void* x16, int x_ld, in
                       int rows, int split, float* dw, float* db, float* dw_hi, float* db_hi, int* nonfinite,
                       void* workspace, size_t workspace_bytes, sb_stream_t stream);
 
+/* ------------------------------------------------- backward pass of the R-CNN heads ----
+ * Together with sb_conv2d_tc_dgrad / sb_conv_wgrad these replace the autograd of lib/model/stereo_rcnn/resnet.py:256-286
+ * (RCNN_top, RCNN_kpts, kpts_class, RCNN_cls_score, RCNN_bbox_pred, RCNN_dim_orien_pred) and stereo_rcnn.py:252-271.
+ * Every reduction runs in a fixed order (bit-identical run to run); *nonfinite (device int, may be NULL) is set to 1
+ * when a result is not finite (never cleared).  Every argument check returns SB_EINVAL before any launch.
+ * sb_box_tail_scores -- sb_box_tail that also writes the raw class scores cls_score [R,nc] the loss reads (cls_prob,
+ *   bbox_pred and dim_orien are the same bits as sb_box_tail's).
+ * sb_kpts_logits -- the keypoint logits [R,6,G] (sb_kpts_tail's kpts_pred_all) split into the loss's kpts_pred [R,4G]
+ *   (channels 0..3), left_border_pred [R,G] (4) and right_border_pred [R,G] (5).
+ * sb_dropout_words -- Dropout(p) in training mode with explicit random words instead of torch's RNG: x[i] (n fp32, or
+ *   fp16 when x_is_half) becomes 0 where words[i] < p 2^32 (as uint32) and x[i] / (1 - p) elsewhere, in place;
+ *   0 <= p < 1.
+ * sb_box_tail_backward -- the three linears on fc7 [R,K] (the saved post-ReLU, post-dropout activation):
+ *   dW / db of RCNN_cls_score [nc,K] / [nc], RCNN_bbox_pred [6nc,K] / [6nc], RCNN_dim_orien_pred [5nc,K] / [5nc] from
+ *   the loss gradients d_cls_score [R,nc], d_bbox_pred [R,6nc], d_dim_orien_pred [R,5nc] (fp32 throughout), and the
+ *   gradient of RCNN_top.3's pre-activation dz32 [R,K] = grad_scale * mask_scale * [fc7 > 0] * sum_o d[r][o] W[o][k]
+ *   (mask_scale = 1 / (1 - p) with dropout, else 1) with its fp16 rounding dz16.  R >= 1, 1 <= n_classes <= 4.
+ * sb_kpts_tail_backward -- the keypoint tail (the deconv output up16 [R,G,G,C] fp16, post-ReLU, summed over height,
+ *   then kpts_class w [6][C]) from d_kpts_pred [R,4G], d_left_border_pred [R,G], d_right_border_pred [R,G]:
+ *   dw [6][C] and db [6] of kpts_class, db_up [C] = the deconv bias gradient (sum over all four phases), and dup16 the
+ *   gradient of the deconv output masked by up16 > 0, times grad_scale, fp16, phase-major [R,G/2,G/2,4C]: pixel (y, x)
+ *   at (y/2, x/2), channels ((y%2)*2 + x%2)*C + c.  G even, 2 <= G <= 64; C % 32 == 0, 32 <= C <= 1024; workspace of
+ *   sb_kpts_tail_backward_workspace bytes.
+ * sb_permute3 -- dst[i0 s0 + i1 s1 + i2 s2] = src[(i0 d1 + i1) d2 + i2] (fp32, out of place): a weight gradient into the
+ *   reference's layout.  The strides must lay the three dimensions out densely in some order.               */
+int sb_box_tail_scores(const float* fc7, int R, int K, int n_classes, const float* w_cls, const float* b_cls,
+                       const float* w_box, const float* b_box, const float* w_dim, const float* b_dim,
+                       float* cls_prob, float* bbox_pred, float* dim_orien, float* cls_score, sb_stream_t stream);
+int sb_kpts_logits(const float* kpts_pred_all, int R, int G, float* kpts_pred, float* left_border_pred,
+                   float* right_border_pred, sb_stream_t stream);
+int sb_dropout_words(void* x, int x_is_half, long long n, const unsigned* words, double p, sb_stream_t stream);
+int sb_box_tail_backward(const float* d_cls_score, const float* d_bbox_pred, const float* d_dim_orien_pred,
+                         const float* fc7, int R, int K, int n_classes, const float* w_cls, const float* w_box,
+                         const float* w_dim, float mask_scale, float grad_scale, float* dw_cls, float* db_cls,
+                         float* dw_box, float* db_box, float* dw_dim, float* db_dim, void* dz16, float* dz32,
+                         int* nonfinite, sb_stream_t stream);
+size_t sb_kpts_tail_backward_workspace(int R, int C);
+int sb_kpts_tail_backward(const void* up16, int R, int G, int C, const float* w, const float* d_kpts_pred,
+                          const float* d_left_border_pred, const float* d_right_border_pred, float grad_scale,
+                          void* dup16, float* dw, float* db, float* db_up, int* nonfinite, void* workspace,
+                          size_t workspace_bytes, sb_stream_t stream);
+int sb_permute3(const float* src, int d0, int d1, int d2, long long s0, long long s1, long long s2, float* dst,
+                sb_stream_t stream);
+
 /* Diagnostics (tools/conv_trace.py): per-CTA phase timestamps of every following sb_conv2d_tc launch, 16 x u64
  * per CTA and 304 CTA slots per launch, into a caller-owned device buffer of sb_conv_trace_bytes(max_launches)
  * bytes.  buf = NULL switches tracing off.  sb_conv_trace_info(id) gives launch id's {Cin, Cout, kh, M, BLOCK_N, tiles,

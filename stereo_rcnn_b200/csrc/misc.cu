@@ -196,7 +196,7 @@ box_tail_kernel(const float* __restrict__ fc7, int K, int nc, const float* __res
                 const float* __restrict__ b_cls, const float* __restrict__ w_box,
                 const float* __restrict__ b_box, const float* __restrict__ w_dim,
                 const float* __restrict__ b_dim, float* __restrict__ cls_prob,
-                float* __restrict__ bbox_pred, float* __restrict__ dim_orien) {
+                float* __restrict__ bbox_pred, float* __restrict__ dim_orien, float* __restrict__ cls_score) {
     __shared__ float part[8][48];
     __shared__ float outv[48];
     const int r = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -224,6 +224,7 @@ box_tail_kernel(const float* __restrict__ fc7, int K, int nc, const float* __res
         for (int j = 0; j < nc; ++j) s += expf(outv[j] - m);
         for (int j = 0; j < nc; ++j) cls_prob[(size_t)r * nc + j] = expf(outv[j] - m) / s;
     }
+    if (cls_score && tid < nc) cls_score[(size_t)r * nc + tid] = outv[tid];     // the raw logits (training)
     if (tid >= nc && tid < 7 * nc) bbox_pred[(size_t)r * 6 * nc + tid - nc] = outv[tid];
     if (tid >= 7 * nc && tid < n_out) dim_orien[(size_t)r * 5 * nc + tid - 7 * nc] = outv[tid];
 }
@@ -485,7 +486,20 @@ extern "C" int sb_box_tail(const float* fc7, int R, int K, int n_classes, const 
     if (R == 0) return SB_OK;
     if (n_classes < 1 || n_classes > 4) return SB_EINVAL;
     box_tail_kernel<<<R, 256, 0, sb_cs(stream)>>>(fc7, K, n_classes, w_cls, b_cls, w_box, b_box, w_dim, b_dim,
-                                                  cls_prob, bbox_pred, dim_orien);
+                                                  cls_prob, bbox_pred, dim_orien, nullptr);
+    SB_LAUNCHED();
+    SB_CHECK_LAUNCH();
+    return SB_OK;
+}
+
+extern "C" int sb_box_tail_scores(const float* fc7, int R, int K, int n_classes, const float* w_cls,
+                                  const float* b_cls, const float* w_box, const float* b_box, const float* w_dim,
+                                  const float* b_dim, float* cls_prob, float* bbox_pred, float* dim_orien,
+                                  float* cls_score, sb_stream_t stream) {
+    if (R == 0) return SB_OK;
+    if (n_classes < 1 || n_classes > 4 || !cls_score) return SB_EINVAL;
+    box_tail_kernel<<<R, 256, 0, sb_cs(stream)>>>(fc7, K, n_classes, w_cls, b_cls, w_box, b_box, w_dim, b_dim,
+                                                  cls_prob, bbox_pred, dim_orien, cls_score);
     SB_LAUNCHED();
     SB_CHECK_LAUNCH();
     return SB_OK;

@@ -56,6 +56,38 @@ def trainable_rpn_params():
             ("RCNN_rpn.RPN_bbox_pred_left_right.bias", (18,))]
 
 
+def trainable_rcnn_head_params(n_classes=2):
+    """[(name, shape)] of the R-CNN heads' parameters (resnet.py:256-286 of the reference), all trainable: RCNN_top
+    (Conv7x7/7 512 -> 2048, Conv1x1 2048 -> 2048), the three linears on fc7, the six keypoint 3x3 convs, the keypoint
+    deconv (ConvTranspose2d, weight [Cin, Cout, 2, 2]) and kpts_class"""
+    out = [("RCNN_top.0.weight", (2048, 512, 7, 7)), ("RCNN_top.0.bias", (2048,)),
+           ("RCNN_top.3.weight", (2048, 2048, 1, 1)), ("RCNN_top.3.bias", (2048,)),
+           ("RCNN_cls_score.weight", (n_classes, 2048)), ("RCNN_cls_score.bias", (n_classes,)),
+           ("RCNN_bbox_pred.weight", (6 * n_classes, 2048)), ("RCNN_bbox_pred.bias", (6 * n_classes,)),
+           ("RCNN_dim_orien_pred.weight", (5 * n_classes, 2048)), ("RCNN_dim_orien_pred.bias", (5 * n_classes,))]
+    for i in range(0, 12, 2):
+        out += [("RCNN_kpts.%d.weight" % i, (256, 256, 3, 3)), ("RCNN_kpts.%d.bias" % i, (256,))]
+    return out + [("RCNN_kpts.12.weight", (256, 256, 2, 2)), ("RCNN_kpts.12.bias", (256,)),
+                  ("kpts_class.weight", (6, 256, 1, 1)), ("kpts_class.bias", (6,))]
+
+
+# Dropout(p=0.2) after each ReLU of RCNN_top (resnet.py:256-263): active in training, since resnet.train() never puts
+# RCNN_top back in eval mode
+DROPOUT_P = 0.2
+
+
+class HeadsSaved(object):
+    """what StereoRCNNEngine.heads(save_for_backward=True) keeps for heads_backward, all for the R sampled RoIs: the fp16
+    pooled tensors pooled_box [R,7,7,512] and pooled_kpts [R,14,14,256]; top0 [R,1,1,2048] fp16 and fc7 [R,2048] fp32,
+    the outputs of RCNN_top.0 / RCNN_top.3 after ReLU and dropout (y > 0 is the combined mask); kpts, the six fp16
+    outputs of RCNN_kpts.0..10 [R,14,14,256]; up [R,28,28,256] fp16, the deconv's ReLU'd output"""
+    __slots__ = ("R", "dropout", "pooled_box", "pooled_kpts", "top0", "fc7", "kpts", "up")
+
+    def __init__(self, R, dropout, pooled_box, pooled_kpts, top0, fc7, kpts, up):
+        self.R, self.dropout, self.pooled_box, self.pooled_kpts = R, dropout, pooled_box, pooled_kpts
+        self.top0, self.fc7, self.kpts, self.up = top0, fc7, kpts, up
+
+
 class RpnSaved(object):
     """what StereoRCNNEngine.rpn(save_for_backward=True) keeps for rpn_backward: per level the fp16 `cat` buffer
     [B,h,w,1024] (the ReLU'd RPN_Conv outputs of L | R: the heads' input and the ReLU mask) and the fp16 P level
@@ -195,6 +227,10 @@ class StereoRCNNEngine(object):
         wd = sd["RCNN_kpts.12.weight"]                                 # [Cin,Cout,2,2]
         self.deconv = [[PackedConv(wd[:, :, a, b].t().contiguous().reshape(256, 256, 1, 1), None,
                                    sd["RCNN_kpts.12.bias"].contiguous(), 0) for b in range(2)] for a in range(2)]
+        # host weights of the two head convs whose data gradient has its own packing (packed on the device only when
+        # heads_backward is first called): RCNN_top.0 as the forward's 1x1 conv over (ph, pw, c), and the deconv as one
+        # 1x1 conv 256 -> 1024 whose output channel (a, b, co) is phase (a, b) of output channel co
+        self._heads_bwd_src = {"RCNN_top.0": w0, "deconv": wd}
         self.kpts_class = (sd["kpts_class.weight"].reshape(6, 256).contiguous(), sd["kpts_class.bias"].contiguous())
         self.fc = [sd[k].contiguous() for k in ("RCNN_cls_score.weight", "RCNN_cls_score.bias",
                                                 "RCNN_bbox_pred.weight", "RCNN_bbox_pred.bias",
@@ -577,8 +613,18 @@ class StereoRCNNEngine(object):
             dps[_LEVELS[i]] = dp
         return out, dps
 
-    def heads(self, feats, B, rois_l, rois_r, im_h):
-        """stereo_rcnn.py:240-271 on flattened rois [R,5]"""
+    def heads(self, feats, B, rois_l, rois_r, im_h, save_for_backward=False, dropout_words=None):
+        """stereo_rcnn.py:240-271 on flattened rois [R,5].
+        save_for_backward=True (fp16-operand engines) returns (out, HeadsSaved) for heads_backward; out then also holds
+        the raw predictions the R-CNN loss reads: cls_score [R,C], kpts_pred [R,4G], left_border_pred and
+        right_border_pred [R,G].  Every other output is the same bits either way.
+        dropout_words (int32 [2,R,2048], train.random_words; fp16-operand engines) applies the training-mode
+        Dropout(p=0.2) after each ReLU of RCNN_top: element i of RCNN_top.0's output (words[0]) and of fc7 (words[1])
+        is dropped when its word, read as uint32, is < 0.2 2^32, and scaled by 1.25 otherwise.  The explicit words
+        replace torch's RNG stream, as the samplers' do (DESIGN 4.4): the one deliberate difference from the
+        reference's dropout."""
+        if (save_for_backward or dropout_words is not None) and not self.half:
+            raise ValueError("the backward pass runs on fp16 conv operands: build the engine with precision='fp16'")
         mk = ("p2", "p3", "p4", "p5")
         fl = [feats[k][:B] for k in mk]
         fr = [feats[k][B:] for k in mk]
@@ -588,26 +634,49 @@ class StereoRCNNEngine(object):
         adt = torch.float16 if h else torch.float32
         rt = not self.exact and not h
         c16 = dict(f32=False, f16=True) if h else {}
+        if dropout_words is not None:
+            assert dropout_words.dtype == torch.int32 and dropout_words.is_contiguous()
+            assert tuple(dropout_words.shape) == (2, R, 2048) and dropout_words.is_cuda
+        nc = self.n_classes
+        # saved for the backward and read by the loss: allocated here on the current stream, not inside the side-stream
+        # fork below
+        train = None
+        if save_for_backward:
+            f32 = lambda *sh: torch.empty(*sh, dtype=torch.float32, device=dev)
+            train = dict(pooled=torch.empty(R, 7, 7, 512, dtype=adt, device=dev),
+                         top0=torch.empty(R, 1, 1, 2048, dtype=adt, device=dev), fc7=f32(R, 1, 1, 2048),
+                         tail=(f32(R, nc), f32(R, 6 * nc), f32(R, 5 * nc), f32(R, nc)))
+
         def box_head():
-            pooled = torch.empty(R, 7, 7, 512, dtype=adt, device=dev)
+            pooled = train["pooled"] if train else torch.empty(R, 7, 7, 512, dtype=adt, device=dev)
             ops.roi_align_pyramid_nhwc(fl, im_h, rois_l, 7, out=pooled, out_coff=0, round_tf32=rt, half=h)
             ops.roi_align_pyramid_nhwc(fr, im_h, rois_r, 7, out=pooled, out_coff=256, round_tf32=rt, half=h)
+            top0 = dict(out16=train["top0"]) if train else {}
             x = self._conv(pooled.view(R, 1, 1, 7 * 7 * 512), self.p["RCNN_top.0"], relu=True, tag="top0",
-                           out_mode=ops.ROUND_TF32, **c16)
-            fc7 = self._conv(x, self.p["RCNN_top.3"], relu=True, tag="top3").view(R, 2048)
-            return (pooled, fc7) + tuple(ops.box_tail(fc7, *self.fc, n_classes=self.n_classes))
+                           out_mode=ops.ROUND_TF32, **c16, **top0)
+            if dropout_words is not None:
+                ops.dropout_words_(x, dropout_words[0], DROPOUT_P)
+            fc7 = self._conv(x, self.p["RCNN_top.3"], relu=True, tag="top3",
+                             out=train["fc7"] if train else None).view(R, 2048)
+            if dropout_words is not None:
+                ops.dropout_words_(fc7, dropout_words[1], DROPOUT_P)
+            if train:
+                return (pooled, fc7, x) + ops.box_tail_scores(fc7, *self.fc, n_classes=nc, out=train["tail"])
+            return (pooled, fc7, x) + tuple(ops.box_tail(fc7, *self.fc, n_classes=nc)) + (None,)
         fork = self.side is not None and self.forks
         if fork:    # the box head (two FCs with 3 row tiles) is latency-bound: run it beside the keypoint convs
             main = torch.cuda.current_stream()
             self.side.wait_stream(main)
             with torch.cuda.stream(self.side):
-                pooled, fc7, cls_prob, bbox, dim = box_head()
+                pooled, fc7, top0, cls_prob, bbox, dim, score = box_head()
         else:
-            pooled, fc7, cls_prob, bbox, dim = box_head()
+            pooled, fc7, top0, cls_prob, bbox, dim, score = box_head()
         pk = ops.roi_align_pyramid_nhwc(fl, im_h, rois_l, 14, round_tf32=rt, half=h)
         x = pk
+        kpts = []
         for i in range(0, 12, 2):
             x = self._conv(x, self.p["RCNN_kpts.%d" % i], relu=True, tag="kpts%d" % i, out_mode=ops.ROUND_TF32, **c16)
+            kpts.append(x)
         up = torch.empty(R, 28, 28, 256, dtype=adt, device=dev)
         for a in range(2):
             for b in range(2):
@@ -617,9 +686,93 @@ class StereoRCNNEngine(object):
         kp, lb, rb, ka = ops.kpts_tail(up, *self.kpts_class, want_pred_all=True)
         if fork:
             main.wait_stream(self.side)
-        return dict(pooled_box=pooled, pooled_kpts=pk, fc7=fc7, cls_prob=cls_prob, bbox_pred=bbox,
-                    dim_orien_pred=dim, kpts_prob=kp, left_border_prob=lb, right_border_prob=rb,
-                    kpts_pred_all=ka)
+        out = dict(pooled_box=pooled, pooled_kpts=pk, fc7=fc7, cls_prob=cls_prob, bbox_pred=bbox,
+                   dim_orien_pred=dim, kpts_prob=kp, left_border_prob=lb, right_border_prob=rb,
+                   kpts_pred_all=ka)
+        if not save_for_backward:
+            return out
+        kpred, lpred, rpred = ops.kpts_logits(ka)
+        out.update(cls_score=score, kpts_pred=kpred, left_border_pred=lpred, right_border_pred=rpred)
+        return out, HeadsSaved(R, dropout_words is not None, pooled, pk, top0, fc7, kpts, up)
+
+    # ------------------------------------------------------------------ backward of the R-CNN heads
+    def _pack_heads_backward(self):
+        self._pack_backward()
+        if "RCNN_top.0" not in self._bwd:
+            w0, wd = self._heads_bwd_src["RCNN_top.0"], self._heads_bwd_src["deconv"]
+            self._bwd["RCNN_top.0"] = _DgradConv(_pack_conv(w0).reshape(2048, 7 * 7 * 512, 1, 1), None, 0, self.device)
+            # deconv as a 1x1 conv with output channel (a, b, co): W[(a, b, co)][ci] = wd[ci, co, a, b]
+            self._bwd["deconv"] = _DgradConv(wd.permute(2, 3, 1, 0).reshape(1024, 256, 1, 1), None, 0, self.device)
+
+    def heads_backward(self, saved, d_cls_score, d_bbox_pred, d_dim_orien_pred, d_kpts_pred, d_left_border_pred,
+                       d_right_border_pred, grads=None, grad_scale=1.0):
+        """Backward of heads (resnet.py:256-286, stereo_rcnn.py:252-271) for the R-CNN loss gradients w.r.t. the raw
+        predictions heads(save_for_backward=True) returns: d_cls_score [R,C], d_bbox_pred [R,6C], d_dim_orien_pred
+        [R,5C], d_kpts_pred [R,4G], d_left_border_pred / d_right_border_pred [R,G] (fp32).
+        Returns ({state_dict name: fp32 gradient} of exactly trainable_rcnn_head_params(n_classes), in the reference's
+        layout; tensors given in `grads` are written in place,
+        {"pooled_box": fp32 [R,7,7,512] (channels 0..255 the left image, 256..511 the right),
+         "pooled_kpts": fp32 [R,14,14,256]}: the gradients of the two pooled tensors).
+        Every sum runs in a fixed order: bit-identical run to run.  grad_scale (a power of two) scales the fp16 chain
+        and is divided out of every result exactly; found_inf is cleared, then set when a gradient is not finite.
+        No host synchronisation: graph-capturable."""
+        self._pack_heads_backward()
+        dev = self.device
+        gs = float(grad_scale)
+        R = saved.R
+        out = self._grad_buffers(trainable_rcnn_head_params(self.n_classes), grads)
+        nf = self._found_inf
+        ops.fill_(nf, 0.0)
+        f32 = lambda *sh: torch.empty(*sh, dtype=torch.float32, device=dev)
+        # the dgrad epilogue's per-channel scale divides grad_scale out of the pooled gradients (exact: a power of two)
+        unscale = ops.fill_(f32(2048), 1.0 / gs) if gs != 1.0 else None
+        # ---- box head: the three linears (fp32), then RCNN_top.3 and RCNN_top.0 as 1x1 convs over the R RoIs
+        keep = 1.0 / (1.0 - DROPOUT_P) if saved.dropout else 1.0
+        w_cls, _, w_box, _, w_dim, _ = self.fc
+        tail = [out[k + s] for k in ("RCNN_cls_score", "RCNN_bbox_pred", "RCNN_dim_orien_pred")
+                for s in (".weight", ".bias")]
+        dz16, dz32 = ops.box_tail_backward(d_cls_score, d_bbox_pred, d_dim_orien_pred, saved.fc7, w_cls, w_box, w_dim,
+                                           tail, mask_scale=keep, grad_scale=gs, nonfinite=nf)
+        dz16, dz32 = dz16.view(R, 1, 1, 2048), dz32.view(R, 1, 1, 2048)
+        self._wgrad(out, "RCNN_top.3", dz16, saved.top0, gs, dy32=dz32)
+        # RCNN_top.0's pre-activation: top3^T dz where the saved post-dropout output is > 0 (ReLU and dropout mask),
+        # times the dropout's 1 / (1 - p)
+        t3 = self._bwd["RCNN_top.3"]
+        d0_32, d0_16 = f32(R, 1, 1, 2048), torch.empty(R, 1, 1, 2048, dtype=torch.float16, device=dev)
+        keep_v = ops.fill_(f32(2048), keep) if saved.dropout else None
+        ops.conv2d_dgrad(ops.conv_desc(dz16, t3.w16, d0_32, t3.Cin, t3.Cout, 1, 1, 1, 0, 1, 1, scale=keep_v,
+                                       out16=d0_16), saved.top0)
+        pooled16 = saved.pooled_box.view(R, 1, 1, 7 * 7 * 512)
+        g0 = f32(2048, 7 * 7 * 512, 1, 1)       # [co][(ph, pw, c)] -> the reference's [co][c][ph][pw] below
+        ops.conv_wgrad(d0_16, pooled16, 1, g0, grad_scale=gs, dy32=d0_32, db=out["RCNN_top.0.bias"], nonfinite=nf)
+        ops.permute3(g0, (2048, 49, 512), (49 * 512, 1, 49), out["RCNN_top.0.weight"])
+        # d pooled_box = top0^T d0, in column blocks of at most 2048 output channels (the conv kernel's widest tile row)
+        t0 = self._bwd["RCNN_top.0"]
+        d_pooled = f32(R, 7, 7, 512)
+        K0 = 7 * 7 * 512
+        for c0 in range(0, K0, 2048):
+            n = min(2048, K0 - c0)
+            ops.conv2d_dgrad(ops.conv_desc(d0_16, t0.w16[c0:c0 + n], d_pooled, 2048, n, 1, 1, 1, 0, 1, 1,
+                                           scale=unscale, out_coff=c0, out_strides=(K0, K0, K0)))
+        # ---- keypoint head: kpts_class over the height-summed deconv output (fp32), the deconv, six 3x3 convs
+        dup16 = ops.kpts_tail_backward(saved.up, self.kpts_class[0], d_kpts_pred, d_left_border_pred,
+                                       d_right_border_pred, out["kpts_class.weight"], out["kpts_class.bias"],
+                                       out["RCNN_kpts.12.bias"], grad_scale=gs, nonfinite=nf)
+        x6 = saved.kpts[5]
+        gd = f32(1024, 256, 1, 1)                   # [(a, b, co)][ci] -> the reference's [ci][co][a][b] below
+        ops.conv_wgrad(dup16, x6, 1, gd, grad_scale=gs, nonfinite=nf)
+        ops.permute3(gd, (4, 256, 256), (1, 4, 1024), out["RCNN_kpts.12.weight"])
+        g32, g16 = self._dgrad(dup16, "deconv", mask=x6)
+        for i in range(5, -1, -1):
+            key = "RCNN_kpts.%d" % (2 * i)
+            xin = saved.kpts[i - 1] if i > 0 else saved.pooled_kpts
+            self._wgrad(out, key, g16, xin, gs, dy32=g32)
+            if i > 0:
+                g32, g16 = self._dgrad(g16, key, mask=xin)
+        pc = self._bwd["RCNN_kpts.0"]
+        d_pk = f32(R, 14, 14, 256)
+        ops.conv2d_dgrad(ops.conv_desc(g16, pc.w16, d_pk, pc.Cin, pc.Cout, 3, 3, 1, 1, 14, 14, scale=unscale))
+        return out, {"pooled_box": d_pooled, "pooled_kpts": d_pk}
 
     @torch.no_grad()
     def forward(self, im_left, im_right, im_info, cfg_key="TEST", keep_features=False, im_h=None,

@@ -91,6 +91,15 @@ _SIGS = {
     "sb_conv_wgrad_acc_workspace": (c_size_t, [c_int] * 6),
     "sb_conv_wgrad_acc": (c_int, [c_void_p, c_int, c_void_p] + [c_int] * 7 + [c_void_p, c_float, c_void_p] +
                           [c_int] * 4 + [c_void_p] * 6 + [c_size_t, c_void_p]),
+    "sb_box_tail_scores": (c_int, [c_void_p, c_int, c_int, c_int] + [c_void_p] * 10 + [c_void_p]),
+    "sb_kpts_logits": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "sb_dropout_words": (c_int, [c_void_p, c_int, c_ll, c_void_p, c_double, c_void_p]),
+    "sb_box_tail_backward": (c_int, [c_void_p] * 4 + [c_int, c_int, c_int] + [c_void_p] * 3 + [c_float, c_float] +
+                             [c_void_p] * 9 + [c_void_p]),
+    "sb_kpts_tail_backward_workspace": (c_size_t, [c_int, c_int]),
+    "sb_kpts_tail_backward": (c_int, [c_void_p, c_int, c_int, c_int] + [c_void_p] * 4 + [c_float] + [c_void_p] * 6 +
+                              [c_size_t, c_void_p]),
+    "sb_permute3": (c_int, [c_void_p, c_int, c_int, c_int, c_ll, c_ll, c_ll, c_void_p, c_void_p]),
     "sb_conv_trace_bytes": (c_size_t, [c_int]),
     "sb_conv_trace": (c_int, [c_void_p, c_int]),
     "sb_conv_trace_count": (c_int, []),

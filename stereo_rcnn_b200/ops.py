@@ -595,6 +595,94 @@ def box_tail(fc7, w_cls, b_cls, w_box, b_box, w_dim, b_dim, n_classes):
     return cls_prob, bbox, dim
 
 
+def box_tail_scores(fc7, w_cls, b_cls, w_box, b_box, w_dim, b_dim, n_classes, out=None):
+    """box_tail plus the raw class scores the loss reads -> cls_prob, bbox_pred, dim_orien, cls_score [R,nc]
+    (out: the four tensors to write, else allocated)"""
+    L = _l.load()
+    R, K = fc7.shape
+    dev = fc7.device
+    if out is None:
+        out = [torch.empty(R, n * n_classes, dtype=torch.float32, device=dev) for n in (1, 6, 5, 1)]
+    cls_prob, bbox, dim, score = out
+    for t, n in zip(out, (1, 6, 5, 1)):
+        assert tuple(t.shape) == (R, n * n_classes) and t.dtype == torch.float32
+    check(L.sb_box_tail_scores(ptr(fc7), R, K, n_classes, ptr(w_cls), ptr(b_cls), ptr(w_box), ptr(b_box), ptr(w_dim),
+                               ptr(b_dim), ptr(cls_prob), ptr(bbox), ptr(dim), ptr(score), stream_ptr()),
+          "sb_box_tail_scores")
+    return cls_prob, bbox, dim, score
+
+
+def kpts_logits(pred_all):
+    """keypoint logits [R,6,G] -> kpts_pred [R,4G], left_border_pred [R,G], right_border_pred [R,G]"""
+    L = _l.load()
+    R, _, G = pred_all.shape
+    dev = pred_all.device
+    kp = torch.empty(R, 4 * G, dtype=torch.float32, device=dev)
+    lb = torch.empty(R, G, dtype=torch.float32, device=dev)
+    rb = torch.empty(R, G, dtype=torch.float32, device=dev)
+    check(L.sb_kpts_logits(ptr(_f32c(pred_all)), R, G, ptr(kp), ptr(lb), ptr(rb), stream_ptr()), "sb_kpts_logits")
+    return kp, lb, rb
+
+
+def dropout_words_(x, words, p):
+    """training-mode Dropout(p) in place on a contiguous fp16 / fp32 tensor: zero where the int32 word, read as uint32,
+    is < p 2^32, x / (1 - p) elsewhere (one word per element)"""
+    L = _l.load()
+    assert x.dtype in (torch.float16, torch.float32) and words.dtype == torch.int32
+    assert words.is_contiguous() and words.numel() == x.numel() and words.device == x.device
+    check(L.sb_dropout_words(ptr(x), 1 if x.dtype == torch.float16 else 0, x.numel(), ptr(words), float(p),
+                             stream_ptr()), "sb_dropout_words")
+    return x
+
+
+def box_tail_backward(d_cls, d_box, d_dim, fc7, w_cls, w_box, w_dim, grads, mask_scale=1.0, grad_scale=1.0,
+                      nonfinite=None):
+    """backward of the box tail's three linears: grads = (dw_cls, db_cls, dw_box, db_box, dw_dim, db_dim), written in
+    place -> (dz16, dz32) [R,K], the gradient of RCNN_top.3's pre-activation times grad_scale"""
+    L = _l.load()
+    R, K = fc7.shape
+    nc = d_cls.shape[1]
+    assert tuple(d_box.shape) == (R, 6 * nc) and tuple(d_dim.shape) == (R, 5 * nc) and d_cls.shape[0] == R
+    for g, n in zip(grads, (nc * K, nc, 6 * nc * K, 6 * nc, 5 * nc * K, 5 * nc)):
+        assert g.dtype == torch.float32 and g.is_contiguous() and g.numel() == n
+    dz16 = torch.empty(R, K, dtype=torch.float16, device=fc7.device)
+    dz32 = torch.empty(R, K, dtype=torch.float32, device=fc7.device)
+    check(L.sb_box_tail_backward(ptr(_f32c(d_cls)), ptr(_f32c(d_box)), ptr(_f32c(d_dim)), ptr(_f32c(fc7)), R, K, nc,
+                                 ptr(w_cls), ptr(w_box), ptr(w_dim), float(mask_scale), float(grad_scale),
+                                 *[ptr(g) for g in grads], ptr(dz16), ptr(dz32), ptr(nonfinite), stream_ptr()),
+          "sb_box_tail_backward")
+    return dz16, dz32
+
+
+def kpts_tail_backward(up16, w, d_kpts_pred, d_left, d_right, dw, db, db_up, grad_scale=1.0, nonfinite=None):
+    """backward of the keypoint tail: up16 [R,G,G,C] the saved deconv output, w [6,C] kpts_class -> dw [6*C], db [6],
+    db_up [C] written in place; returns dup16 [R,G/2,G/2,4C], the masked deconv-output gradient times grad_scale in
+    the deconv's four (a, b) phases"""
+    L = _l.load()
+    R, G, _, C = up16.shape
+    assert up16.dtype == torch.float16 and up16.is_contiguous()
+    assert tuple(d_kpts_pred.shape) == (R, 4 * G) and tuple(d_left.shape) == (R, G) and tuple(d_right.shape) == (R, G)
+    for g, n in ((dw, 6 * C), (db, 6), (db_up, C)):
+        assert g.dtype == torch.float32 and g.is_contiguous() and g.numel() == n
+    dup = torch.empty(R, G // 2, G // 2, 4 * C, dtype=torch.float16, device=up16.device)
+    nb = L.sb_kpts_tail_backward_workspace(R, C)
+    ws = workspace(nb, up16.device, "kpts_tail_bwd")
+    check(L.sb_kpts_tail_backward(ptr(up16), R, G, C, ptr(w), ptr(_f32c(d_kpts_pred)), ptr(_f32c(d_left)),
+                                  ptr(_f32c(d_right)), float(grad_scale), ptr(dup), ptr(dw), ptr(db), ptr(db_up),
+                                  ptr(nonfinite), ptr(ws), nb, stream_ptr()), "sb_kpts_tail_backward")
+    return dup
+
+
+def permute3(src, dims, strides, dst):
+    """dst[i0 s0 + i1 s1 + i2 s2] = src[i0, i1, i2] for src viewed as dims = (d0, d1, d2) (fp32, out of place)"""
+    L = _l.load()
+    assert src.dtype == torch.float32 and dst.dtype == torch.float32 and dst.is_contiguous()
+    assert src.numel() == dst.numel() == dims[0] * dims[1] * dims[2]
+    check(L.sb_permute3(ptr(_f32c(src)), *[int(d) for d in dims], *[int(s) for s in strides], ptr(dst), stream_ptr()),
+          "sb_permute3")
+    return dst
+
+
 def test_decode(rois_left, rois_right, bbox_pred, dim_orien, kpts_prob, left_prob, right_prob, im_info,
                 n_classes=2, grid=28):
     """test_net.py:138-212 -> pred_boxes_left [R,4nc], pred_boxes_right, dim_orien [R,5nc], pred_kpts [R,5]"""

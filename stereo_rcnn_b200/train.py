@@ -5,7 +5,8 @@ Host-side mirror of `_AnchorTargetLayer` (lib/model/rpn/anchor_target_layer.py:4
 stereo_rcnn.py:201-311), the multi-task sum (trainval_net.py:214-219) and `clip_gradient` (net_utils.py:37-49) over
 libstereo_b200's kernels (csrc/train_targets.cu, csrc/train_loss.cu).  No host synchronisation anywhere: counts,
 sampled indices and losses stay on the device.  rpn_gradients composes them with the engine's forward and backward
-passes into the gradients of the RPN loss for the trunk, the FPN and the RPN.
+passes into the gradients of the RPN loss for the trunk, the FPN and the RPN, and rcnn_head_gradients into the gradients
+of the R-CNN loss for the heads.
 """
 import ctypes
 
@@ -203,3 +204,50 @@ def rpn_gradients(engine, im_left, im_right, gt_left, gt_right, gt_merge, keys, 
             return losses, g
         _total, d_u = multitask_loss(losses, u)
         return losses, g, d_u
+
+
+_IM_INFO = {}
+
+
+def _im_info(B, H, W, device):
+    """im_info [B,3] = (H, W, 1) on the device, built once per (device, B, H, W): later calls, and CUDA graphs captured
+    after a first eager call, read the same tensor (the proposal layer reads only H and W)"""
+    key = (str(device), B, H, W)
+    if key not in _IM_INFO:
+        _IM_INFO[key] = torch.tensor([[float(H), float(W), 1.0]] * B, dtype=torch.float32).to(device)
+    return _IM_INFO[key]
+
+
+def rcnn_head_gradients(engine, im_left, im_right, gt_left, gt_right, gt_merge, gt_dim_orien, gt_kpts, keys, words,
+                        dropout_words=None, uncert=None, grads=None, grad_scale=1.0):
+    """The R-CNN loss of a stereo pair differentiated through the heads on a frozen trunk and RPN
+    (stereo_rcnn.py:198-311): trunk_fpn and rpn (no gradient), proposal_layer(..., "TRAIN"), proposal_targets for
+    `keys` [B,R+K] / `words` [B,S], heads(save_for_backward=True) on the S sampled RoIs per image, rcnn_loss, then
+    heads_backward.  im_left / im_right [B,3,H,W] NCHW fp32 network inputs, gt_* [B,K,5], gt_dim_orien [B,K,5],
+    gt_kpts [B,K,6]; gt_merge is part of the ground truth of a step but only the RPN's targets read it.
+    dropout_words (int32 [2,B*S,2048], random_words): RCNN_top's training-mode dropout (engine.heads).
+    Returns (losses [4] = (RCNN_loss_cls, RCNN_loss_bbox, RCNN_loss_dim_orien, RCNN_loss_kpts),
+    {state_dict name: fp32 gradient} of trainable_rcnn_head_params(n_classes),
+    {"pooled_box": [B*S,7,7,512], "pooled_kpts": [B*S,14,14,256]} fp32 gradients of the pooled features) and, with
+    uncert [6] (the multi-task weights of trainval_net.py:214-219; uncert[2:6] weight these four losses),
+    d total / d uncert[2:6] as a fourth item; the gradients are then those of losses[i] * exp(-uncert[2 + i]).
+    grads / grad_scale as in heads_backward.  No optimizer step, no host synchronisation."""
+    B, _, H, W = im_left.shape
+    with torch.no_grad():
+        im = torch.cat((im_left, im_right), 0).contiguous()
+        feats = engine.trunk_fpn(im)
+        cls_prob, bbox, shapes = engine.rpn(feats, B)
+        from .ops import proposal_layer
+        rl, rr = proposal_layer(cls_prob, bbox, _im_info(B, H, W, im.device), "TRAIN", shapes)
+        tgt = proposal_targets(rl, rr, gt_left, gt_right, gt_dim_orien, gt_kpts, keys, words)
+        out, saved = engine.heads(feats, B, tgt["rois_left"].view(-1, 5), tgt["rois_right"].view(-1, 5), float(H),
+                                  save_for_backward=True, dropout_words=dropout_words)
+        # sb_rcnn_loss reads uncert[2..5] of the whole vector
+        losses, g = rcnn_loss(out["cls_score"], out["bbox_pred"], out["dim_orien_pred"], out["kpts_pred"],
+                              out["left_border_pred"], out["right_border_pred"], tgt, uncert=uncert)
+        hg, dpooled = engine.heads_backward(saved, *g, grads=grads, grad_scale=grad_scale)
+        if uncert is None:
+            return losses, hg, dpooled
+        assert uncert.numel() >= 6
+        _total, d_u = multitask_loss(losses, uncert[2:6])
+        return losses, hg, dpooled, d_u
