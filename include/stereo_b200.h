@@ -92,6 +92,34 @@ int sb_roi_align_pyramid_nhwc(const float* const* feats, const int* heights, con
                               int C, float im_h, const float* rois, int R, int pooled,
                               float* out, int out_ld, int out_coff, int round_tf32, sb_stream_t stream);
 
+/* Backward of sb_roi_align_pyramid_nhwc (mode 0) for fp32 gradients: the exact adjoint of the forward, routing and
+ * taps included, ADDED in place into fp32 NHWC level gradients dfeats[l] [N, H_l, W_l, C] (l = P2..P5).
+ * A source is one forward call's gradient: grad[r][ph][pw][coff + c] (row pitch ld) of RoI r of rois [R,5], pooled =
+ * P, read at image batch_offset + rois[r][0] of the levels (0 for the left images, B for the right ones).
+ * Lattice point gradient gl = ((G[i-1][j-1] + G[i-1][j]) + (G[i][j-1] + G[i][j])) / 4 in fp64 over the outputs that
+ * read it; each corner of its bilinear tap (the forward's fp64 weights; zero taps contribute nothing) gains
+ * rint(gl 2^e w) in a 64-bit fixed-point accumulator, e = 60 - ex - k with max|G| < 2^ex over every source and
+ * T = sum_s R_s (P_s+1)^2 <= 2^k the call's lattice taps (at most T contributions per element: no overflow).
+ * Finally dfeats += acc 2^-e in fp64, one rounding to fp32.  Bit-identical run to run and under any permutation of
+ * the RoIs of a source.  Per element, |result - exact| <= 2^-e n + ulp/2 (+ fp64 rounding), n its contributions.
+ * *nonfinite (device int, may be NULL) is set to 1 when a gradient read or a result is not finite (never cleared);
+ * a non-finite gradient makes every element of dfeats NaN.  A RoI whose image lies outside [0, N) contributes
+ * nothing.  Workspace: sb_roi_align_pyramid_backward_workspace bytes, 8-byte aligned.
+ * SB_EINVAL, before any launch, unless: 1 <= n_sources <= 4; N >= 1; C > 0 and C % 4 == 0; every level has a
+ * non-null pointer and H_l >= 2, W_l >= 2; the workspace is non-null, aligned and large enough; and for each source
+ * R >= 0, pooled >= 1, ld % 4 == 0, coff >= 0, coff % 4 == 0, coff + C <= ld, 0 <= batch_offset < N, grad and
+ * rois non-null when R > 0, and (rb+1)(pooled+1) 40 bytes of shared memory <= 48 KB (rb as the forward's).
+ * R == 0 in every source launches nothing and leaves dfeats untouched.                                        */
+typedef struct {
+    const float* grad;
+    const float* rois;
+    int R, pooled, ld, coff, batch_offset;
+} sb_roi_grad_source;
+size_t sb_roi_align_pyramid_backward_workspace(const int* heights, const int* widths, int N, int C);
+int sb_roi_align_pyramid_backward(const sb_roi_grad_source* sources, int n_sources, float* const* dfeats,
+                                  const int* heights, const int* widths, int N, int C, float im_h,
+                                  int* nonfinite, void* workspace, size_t workspace_bytes, sb_stream_t stream);
+
 /* ----------------------------------------------------- proposal layer ----
  * cls_prob [B,A,2] (column 1 = score), bbox_pred_lr [B,A,6], im_info [B,3] (device).
  * cfg: host struct (anchor pyramid + top-N / threshold constants), A = n_ratios*sum(h*w).

@@ -269,6 +269,158 @@ roi_align_pyramid_nhwc(PyramidArgs a, int C, const float* __restrict__ rois, int
     }
 }
 
+// ---- backward of roi_align_pyramid_nhwc: the exact adjoint, accumulated deterministically (SURVEY 7.8).
+// Lattice point (lr, lc) of a RoI is read by the outputs (lr-1 | lr, lc-1 | lc) that exist, each with weight 1/4, so its
+// gradient is gl = ((G[lr-1][lc-1] + G[lr-1][lc]) + (G[lr][lc-1] + G[lr][lc])) * 0.25 (fp64, absent outputs are 0).  Each
+// corner of its bilinear tap receives rint(gl * 2^e * w) in a 64-bit fixed-point accumulator per level element; integer
+// addition is associative, so the result depends neither on the order of the atomics nor on the order of the RoIs.
+// The exponent: |gl| <= max|G| < 2^ex and |w| < 4 (hr, wr < 2 on the extrapolated last row / column), so one
+// contribution is below 2^(ex+2+e) + 1/2; a level element receives at most one contribution per lattice tap of the call
+// (the four corners of a tap are distinct pixels because H, W >= 2), T <= 2^k in all.  e = 60 - ex - k keeps every sum
+// below 2^62 + 2^(k-1) < 2^63.
+constexpr int kMaxGradSources = 4;
+
+struct PyrGradSrc {
+    const float* grad;      // [R, P, P, ld], channels [coff, coff + C)
+    const float* rois;      // [R, 5]
+    int R, P, RB, nblk, ld, coff, boff;
+    int cta0;               // first CTA of this source in the grid
+};
+
+struct PyramidGradArgs {
+    PyrGradSrc src[kMaxGradSources];
+    int n_src;
+    float* dfeat[4];        // [N, H, W, C] fp32 per level
+    int H[4], W[4];
+    float scale[4];
+    long long acc_off[4];   // element offset of each level in the accumulator
+    int N, kbits;
+};
+
+__device__ __forceinline__ int pyramid_grad_exponent(unsigned absmax_bits, int kbits) {
+    int ex;
+    frexpf(__uint_as_float(absmax_bits), &ex);                         // |G| < 2^ex
+    return 60 - ex - kbits;
+}
+
+__device__ __forceinline__ unsigned abs_bits4(float4 v) {
+    const unsigned a = __float_as_uint(v.x) & 0x7fffffffu, b = __float_as_uint(v.y) & 0x7fffffffu;
+    const unsigned c = __float_as_uint(v.z) & 0x7fffffffu, d = __float_as_uint(v.w) & 0x7fffffffu;
+    return max(max(a, b), max(c, d));
+}
+
+// max |G| over every source's channel slice (as bits: monotonic for finite values, inf and nan above them)
+__global__ void __launch_bounds__(256)
+pyramid_grad_absmax(PyramidGradArgs a, int C, unsigned* __restrict__ absmax, int* nonfinite) {
+    const int C4 = C >> 2;
+    unsigned m = 0u;
+    for (int s = 0; s < a.n_src; ++s) {
+        const PyrGradSrc& S = a.src[s];
+        const long long n = (long long)S.R * S.P * S.P * C4;
+        for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+            const long long row = i / C4;
+            const int c4 = (int)(i - row * C4);
+            m = max(m, abs_bits4(__ldg(reinterpret_cast<const float4*>(S.grad + row * S.ld + S.coff) + c4)));
+        }
+    }
+    m = __reduce_max_sync(0xffffffffu, m);
+    if ((threadIdx.x & 31) == 0 && m) {
+        atomicMax(absmax, m);
+        if (m >= 0x7f800000u && nonfinite) *nonfinite = 1;
+    }
+}
+
+__device__ __forceinline__ void fixed_add4(unsigned long long* p, const double (&g)[4], double w) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const long long v = __double2ll_rn(g[j] * w);
+        if (v) atomicAdd(p + j, (unsigned long long)v);                // two's complement: wraps like int64
+    }
+}
+
+// One CTA per (source, RoI, block of RB output rows), as the forward.  The CTA owns lattice rows ph0 .. ph0 + rows - 1
+// (plus row P in the last block): every lattice point is formed once, from all four outputs that read it.
+// dynamic smem = (RB + 1) * (P + 1) tap records.
+__global__ void __launch_bounds__(256)
+roi_align_pyramid_bwd(PyramidGradArgs a, int C, const unsigned* __restrict__ absmax,
+                      unsigned long long* __restrict__ acc) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    TapRec* taps = reinterpret_cast<TapRec*>(smem_raw);
+    const unsigned amax = *absmax;
+    if (amax == 0u || amax >= 0x7f800000u) return;         // no contribution, or non-finite (flagged, dP set to NaN)
+    int s = 0;
+    while (s + 1 < a.n_src && (int)blockIdx.x >= a.src[s + 1].cta0) ++s;
+    const PyrGradSrc& S = a.src[s];
+    const int local = blockIdx.x - S.cta0;
+    const int n = local / S.nblk, ph0 = (local - n * S.nblk) * S.RB;
+    const int P = S.P, L = P + 1, C4 = C >> 2;
+    const int rows = min(S.RB, P - ph0);
+    const int nl = rows + (ph0 + rows == P ? 1 : 0);        // lattice rows owned by this CTA
+    const float* roi = S.rois + 5 * n;
+    const int lv = roi_level(roi);
+    const int H = a.H[lv], W = a.W[lv];
+    const RoiGeom g = roi_geom(roi, a.scale[lv], L, L);
+    const int img = g.batch + S.boff;
+    const bool inside = img >= 0 && img < a.N;              // a RoI of no image of the levels contributes nothing
+    for (int e = threadIdx.x; e < nl * L; e += blockDim.x) {
+        const int r = e / L, pw = e - r * L;
+        const Tap t = make_tap(g, ph0 + r, pw, H, W);
+        TapRec tr;
+        tr.w00 = t.w00; tr.w01 = t.w01; tr.w10 = t.w10; tr.w11 = t.w11;
+        tr.off = (t.zero || !inside) ? -1 : a.acc_off[lv] + (long long)((((size_t)img * H + t.h0) * W + t.w0) * C);
+        taps[e] = tr;
+    }
+    __syncthreads();
+    const double sc = ldexp(0.25, pyramid_grad_exponent(amax, a.kbits));      // the average's 1/4 and 2^e, both exact
+    const float* gb = S.grad + (size_t)n * P * P * S.ld + S.coff;
+    const size_t wstep = (size_t)W * C;
+    const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int e = threadIdx.x; e < nl * L * C4; e += blockDim.x) {
+        const int c4 = e % C4, q = e / C4;
+        const TapRec& t = taps[q];
+        if (t.off < 0) continue;
+        const int lr = ph0 + q / L, lc = q % L;
+        auto ld4 = [&](int ph, int pw) {
+            return __ldg(reinterpret_cast<const float4*>(gb + ((size_t)ph * P + pw) * S.ld) + c4);
+        };
+        const bool up = lr > 0, dn = lr < P, lf = lc > 0, rt = lc < P;
+        const float4 ga = up && lf ? ld4(lr - 1, lc - 1) : z4, gb_ = up && rt ? ld4(lr - 1, lc) : z4;
+        const float4 gc = dn && lf ? ld4(lr, lc - 1) : z4, gd = dn && rt ? ld4(lr, lc) : z4;
+        const double gl[4] = {
+            (((double)ga.x + (double)gb_.x) + ((double)gc.x + (double)gd.x)) * sc,
+            (((double)ga.y + (double)gb_.y) + ((double)gc.y + (double)gd.y)) * sc,
+            (((double)ga.z + (double)gb_.z) + ((double)gc.z + (double)gd.z)) * sc,
+            (((double)ga.w + (double)gb_.w) + ((double)gc.w + (double)gd.w)) * sc};
+        unsigned long long* p = acc + t.off + 4 * c4;
+        fixed_add4(p, gl, t.w00);
+        fixed_add4(p + C, gl, t.w01);
+        fixed_add4(p + wstep, gl, t.w10);
+        fixed_add4(p + wstep + C, gl, t.w11);
+    }
+}
+
+// dP += acc * 2^-e in fp64, one rounding to fp32; non-finite input gradients make every element NaN
+__global__ void __launch_bounds__(256)
+pyramid_grad_finish(PyramidGradArgs a, int C, const unsigned* __restrict__ absmax,
+                    const unsigned long long* __restrict__ acc, int* nonfinite) {
+    const unsigned amax = *absmax;
+    if (amax == 0u) return;                                 // every contribution is zero: dP unchanged
+    const bool bad = amax >= 0x7f800000u;
+    const double inv = bad ? 0.0 : ldexp(1.0, -pyramid_grad_exponent(amax, a.kbits));
+    bool nf = false;
+    for (int l = 0; l < 4; ++l) {
+        const long long n = (long long)a.N * a.H[l] * a.W[l] * C;
+        const unsigned long long* al = acc + a.acc_off[l];
+        float* d = a.dfeat[l];
+        for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+            const float v = bad ? __int_as_float(0x7fffffff) : (float)((double)(long long)al[i] * inv + (double)d[i]);
+            d[i] = v;
+            nf |= !isfinite(v);
+        }
+    }
+    if (nf && nonfinite) *nonfinite = 1;
+}
+
 }  // namespace
 
 extern "C" int sb_roi_align_forward(const float* features, int N, int C, int H, int W, const float* rois,
@@ -364,6 +516,97 @@ extern "C" int sb_roi_align_pyramid_nhwc(const float* const* feats, const int* h
     }
     dim3 grid(R, (pooled + RB - 1) / RB);
     roi_align_pyramid_nhwc<<<grid, 256, smem, sb_cs(stream)>>>(a, C, rois, pooled, RB, out, out_ld, out_coff, round_tf32);
+    SB_LAUNCHED();
+    SB_CHECK_LAUNCH();
+    return SB_OK;
+}
+
+static long long pyramid_grad_elems(const int* heights, const int* widths, int N, int C) {
+    long long n = 0;
+    for (int l = 0; l < 4; ++l) n += (long long)N * heights[l] * widths[l] * C;
+    return n;
+}
+
+extern "C" size_t sb_roi_align_pyramid_backward_workspace(const int* heights, const int* widths, int N, int C) {
+    if (!heights || !widths || N < 1 || C < 1) return 0;
+    for (int l = 0; l < 4; ++l)
+        if (heights[l] < 2 || widths[l] < 2) return 0;
+    return (size_t)pyramid_grad_elems(heights, widths, N, C) * 8 + 16;
+}
+
+extern "C" int sb_roi_align_pyramid_backward(const sb_roi_grad_source* sources, int n_sources, float* const* dfeats,
+                                             const int* heights, const int* widths, int N, int C, float im_h,
+                                             int* nonfinite, void* workspace, size_t workspace_bytes,
+                                             sb_stream_t stream) {
+    // every check before the first CUDA call, with the forward's rules for each source's slice and for the levels
+    if (!sources || n_sources < 1 || n_sources > kMaxGradSources || !dfeats || !heights || !widths || N < 1 ||
+        C <= 0 || (C & 3))
+        return SB_EINVAL;
+    PyramidGradArgs a;
+    for (int l = 0; l < 4; ++l) {
+        if (!dfeats[l] || heights[l] < 2 || widths[l] < 2) return SB_EINVAL;
+        a.dfeat[l] = dfeats[l];
+        a.H[l] = heights[l];
+        a.W[l] = widths[l];
+        a.scale[l] = (float)((double)heights[l] / (double)im_h);      // as the forward
+    }
+    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 7) ||
+        workspace_bytes < sb_roi_align_pyramid_backward_workspace(heights, widths, N, C))
+        return SB_EINVAL;
+    long long taps = 0, ctas = 0;
+    size_t smem = 0;
+    a.n_src = n_sources;
+    for (int s = 0; s < n_sources; ++s) {
+        const sb_roi_grad_source& q = sources[s];
+        if (q.R < 0 || q.pooled < 1 || (q.ld & 3) || q.coff < 0 || (q.coff & 3) || (long long)q.coff + C > q.ld ||
+            q.batch_offset < 0 || q.batch_offset >= N || (q.R > 0 && (!q.grad || !q.rois)))
+            return SB_EINVAL;
+        PyrGradSrc& S = a.src[s];
+        S.grad = q.grad;
+        S.rois = q.rois;
+        S.R = q.R;
+        S.P = q.pooled;
+        S.RB = q.pooled <= 8 ? q.pooled : (q.pooled + 1) / 2;     // the forward's row blocks
+        S.nblk = (q.pooled + S.RB - 1) / S.RB;
+        S.ld = q.ld;
+        S.coff = q.coff;
+        S.boff = q.batch_offset;
+        S.cta0 = (int)ctas;
+        const size_t sm = (size_t)(S.RB + 1) * (q.pooled + 1) * sizeof(TapRec);
+        if (sm > 48 * 1024) return SB_EINVAL;
+        smem = sm > smem ? sm : smem;
+        ctas += (long long)q.R * S.nblk;
+        taps += (long long)q.R * (q.pooled + 1) * (q.pooled + 1);
+        if (ctas > 0x7fffffffLL) return SB_EINVAL;
+    }
+    if (taps == 0) return SB_OK;                            // no RoI: dP untouched, nothing launched
+    int kbits = 0;
+    while ((1LL << kbits) < taps) ++kbits;                  // T <= 2^k contributions per level element
+    a.kbits = kbits;
+    a.N = N;
+    long long off = 0;
+    for (int l = 0; l < 4; ++l) {
+        a.acc_off[l] = off;
+        off += (long long)N * heights[l] * widths[l] * C;
+    }
+    cudaStream_t st = sb_cs(stream);
+    unsigned long long* acc = static_cast<unsigned long long*>(workspace);
+    unsigned* absmax = reinterpret_cast<unsigned*>(acc + off);
+    cudaError_t e = cudaMemsetAsync(workspace, 0, (size_t)off * 8 + 16, st);
+    if (e != cudaSuccess) return (int)e;
+    long long nin = 0;
+    for (int s = 0; s < n_sources; ++s) nin += (long long)sources[s].R * sources[s].pooled * sources[s].pooled * (C / 4);
+    const int gin = (int)(nin < 1 ? 1 : ((nin + 255) / 256 < 1184 ? (nin + 255) / 256 : 1184));
+    pyramid_grad_absmax<<<gin, 256, 0, st>>>(a, C, absmax, nonfinite);
+    SB_LAUNCHED();
+    SB_CHECK_LAUNCH();
+    if (ctas > 0) {
+        roi_align_pyramid_bwd<<<(int)ctas, 256, smem, st>>>(a, C, absmax, acc);
+        SB_LAUNCHED();
+        SB_CHECK_LAUNCH();
+    }
+    const int gout = (int)((off + 255) / 256 < 2368 ? (off + 255) / 256 : 2368);
+    pyramid_grad_finish<<<gout, 256, 0, st>>>(a, C, absmax, acc, nonfinite);
     SB_LAUNCHED();
     SB_CHECK_LAUNCH();
     return SB_OK;

@@ -80,12 +80,15 @@ class HeadsSaved(object):
     """what StereoRCNNEngine.heads(save_for_backward=True) keeps for heads_backward, all for the R sampled RoIs: the fp16
     pooled tensors pooled_box [R,7,7,512] and pooled_kpts [R,14,14,256]; top0 [R,1,1,2048] fp16 and fc7 [R,2048] fp32,
     the outputs of RCNN_top.0 / RCNN_top.3 after ReLU and dropout (y > 0 is the combined mask); kpts, the six fp16
-    outputs of RCNN_kpts.0..10 [R,14,14,256]; up [R,28,28,256] fp16, the deconv's ReLU'd output"""
-    __slots__ = ("R", "dropout", "pooled_box", "pooled_kpts", "top0", "fc7", "kpts", "up")
+    outputs of RCNN_kpts.0..10 [R,14,14,256]; up [R,28,28,256] fp16, the deconv's ReLU'd output; and for
+    roi_align_backward the RoIs the pooling read (rois_l, rois_r [R,5]: references, not copies), im_h and B"""
+    __slots__ = ("R", "dropout", "pooled_box", "pooled_kpts", "top0", "fc7", "kpts", "up", "rois_l", "rois_r", "im_h",
+                 "B")
 
-    def __init__(self, R, dropout, pooled_box, pooled_kpts, top0, fc7, kpts, up):
+    def __init__(self, R, dropout, pooled_box, pooled_kpts, top0, fc7, kpts, up, rois_l, rois_r, im_h, B):
         self.R, self.dropout, self.pooled_box, self.pooled_kpts = R, dropout, pooled_box, pooled_kpts
         self.top0, self.fc7, self.kpts, self.up = top0, fc7, kpts, up
+        self.rois_l, self.rois_r, self.im_h, self.B = rois_l, rois_r, im_h, B
 
 
 class RpnSaved(object):
@@ -693,7 +696,8 @@ class StereoRCNNEngine(object):
             return out
         kpred, lpred, rpred = ops.kpts_logits(ka)
         out.update(cls_score=score, kpts_pred=kpred, left_border_pred=lpred, right_border_pred=rpred)
-        return out, HeadsSaved(R, dropout_words is not None, pooled, pk, top0, fc7, kpts, up)
+        return out, HeadsSaved(R, dropout_words is not None, pooled, pk, top0, fc7, kpts, up, rois_l, rois_r,
+                               float(im_h), B)
 
     # ------------------------------------------------------------------ backward of the R-CNN heads
     def _pack_heads_backward(self):
@@ -705,7 +709,7 @@ class StereoRCNNEngine(object):
             self._bwd["deconv"] = _DgradConv(wd.permute(2, 3, 1, 0).reshape(1024, 256, 1, 1), None, 0, self.device)
 
     def heads_backward(self, saved, d_cls_score, d_bbox_pred, d_dim_orien_pred, d_kpts_pred, d_left_border_pred,
-                       d_right_border_pred, grads=None, grad_scale=1.0):
+                       d_right_border_pred, grads=None, grad_scale=1.0, clear_found_inf=True):
         """Backward of heads (resnet.py:256-286, stereo_rcnn.py:252-271) for the R-CNN loss gradients w.r.t. the raw
         predictions heads(save_for_backward=True) returns: d_cls_score [R,C], d_bbox_pred [R,6C], d_dim_orien_pred
         [R,5C], d_kpts_pred [R,4G], d_left_border_pred / d_right_border_pred [R,G] (fp32).
@@ -714,7 +718,8 @@ class StereoRCNNEngine(object):
         {"pooled_box": fp32 [R,7,7,512] (channels 0..255 the left image, 256..511 the right),
          "pooled_kpts": fp32 [R,14,14,256]}: the gradients of the two pooled tensors).
         Every sum runs in a fixed order: bit-identical run to run.  grad_scale (a power of two) scales the fp16 chain
-        and is divided out of every result exactly; found_inf is cleared, then set when a gradient is not finite.
+        and is divided out of every result exactly; found_inf is cleared, then set when a gradient is not finite;
+        clear_found_inf=False keeps a flag an earlier backward of the same step set (rpn_backward before this).
         No host synchronisation: graph-capturable."""
         self._pack_heads_backward()
         dev = self.device
@@ -722,7 +727,8 @@ class StereoRCNNEngine(object):
         R = saved.R
         out = self._grad_buffers(trainable_rcnn_head_params(self.n_classes), grads)
         nf = self._found_inf
-        ops.fill_(nf, 0.0)
+        if clear_found_inf:
+            ops.fill_(nf, 0.0)
         f32 = lambda *sh: torch.empty(*sh, dtype=torch.float32, device=dev)
         # the dgrad epilogue's per-channel scale divides grad_scale out of the pooled gradients (exact: a power of two)
         unscale = ops.fill_(f32(2048), 1.0 / gs) if gs != 1.0 else None
@@ -773,6 +779,23 @@ class StereoRCNNEngine(object):
         d_pk = f32(R, 14, 14, 256)
         ops.conv2d_dgrad(ops.conv_desc(g16, pc.w16, d_pk, pc.Cin, pc.Cout, 3, 3, 1, 1, 14, 14, scale=unscale))
         return out, {"pooled_box": d_pooled, "pooled_kpts": d_pk}
+
+    def roi_align_backward(self, saved_heads, d_pooled, d_feats):
+        """Backward of the heads' three pyramid RoIAligns (stereo_rcnn.py:110-139): adds the gradients of the pooled
+        tensors, d_pooled = heads_backward's {"pooled_box": [R,7,7,512], "pooled_kpts": [R,14,14,256]} (fp32), into
+        d_feats["p2".."p5"] (fp32 NHWC [2B,h,w,256], e.g. rpn_backward's dP), in place and in one deterministic call:
+        box channels 0..255 with rois_l into the left images, 256..511 with rois_r into the right images, and the
+        keypoint pooling with rois_l into the left images.  Sets found_inf on a non-finite gradient, never clears it.
+        No host synchronisation: graph-capturable.  -> d_feats"""
+        self._pack_backward()
+        s = saved_heads
+        dp = [d_feats[k] for k in ("p2", "p3", "p4", "p5")]
+        C = dp[0].shape[3]          # heads() pools the right image into channels C..2C-1 of pooled_box
+        ops.roi_align_pyramid_backward(dp, s.im_h, [(d_pooled["pooled_box"], s.rois_l, 0, 0),
+                                                    (d_pooled["pooled_box"], s.rois_r, C, s.B),
+                                                    (d_pooled["pooled_kpts"], s.rois_l, 0, 0)],
+                                       nonfinite=self._found_inf)
+        return d_feats
 
     @torch.no_grad()
     def forward(self, im_left, im_right, im_info, cfg_key="TEST", keep_features=False, im_h=None,

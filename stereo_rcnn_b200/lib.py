@@ -42,6 +42,11 @@ class ProposalTargetCfg(ctypes.Structure):
                 ("kpts_grid", c_int)]
 
 
+class RoiGradSource(ctypes.Structure):
+    _fields_ = [("grad", c_void_p), ("rois", c_void_p), ("R", c_int), ("pooled", c_int), ("ld", c_int),
+                ("coff", c_int), ("batch_offset", c_int)]
+
+
 _SIGS = {
     "sb_version": (c_int, []),
     "sb_device_cc": (c_int, []),
@@ -59,6 +64,11 @@ _SIGS = {
     "sb_roi_align_pyramid_nhwc": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_int), ctypes.POINTER(c_int),
                                           c_int, c_float, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int,
                                           c_void_p]),
+    "sb_roi_align_pyramid_backward_workspace": (c_size_t, [ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_int,
+                                                           c_int]),
+    "sb_roi_align_pyramid_backward": (c_int, [ctypes.POINTER(RoiGradSource), c_int, ctypes.POINTER(c_void_p),
+                                              ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_int, c_int, c_float,
+                                              c_void_p, c_void_p, c_size_t, c_void_p]),
     "sb_proposal_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "sb_proposal_layer": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, ctypes.POINTER(ProposalCfg),
                                   c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),

@@ -165,6 +165,39 @@ def roi_align_pyramid_nhwc(feats, im_h, rois, pooled, out=None, out_coff=0, roun
     return out
 
 
+def roi_align_pyramid_backward(d_feats, im_h, sources, nonfinite=None):
+    """backward of roi_align_pyramid_nhwc: adds the gradient of every source into d_feats, 4 NHWC fp32 tensors
+    [N,h,w,C] (P2..P5), in place.  sources: up to 4 tuples (grad [R,P,P,ld] fp32, rois [R,5], coff, batch_offset):
+    channels coff..coff+C of grad are the gradient of a forward call on the levels' images batch_offset + rois[:,0].
+    Deterministic (64-bit fixed point, one exponent for the call); nonfinite: int32 [1] device flag set to 1 on a
+    non-finite gradient or result, never cleared.  -> d_feats"""
+    L = _l.load()
+    assert len(d_feats) == 4 and 1 <= len(sources)
+    N, C = d_feats[0].shape[0], d_feats[0].shape[3]
+    dev = d_feats[0].device
+    for f in d_feats:     # the kernel adds into each level as dense [N, H, W, C] fp32 rows on the RoIs' device
+        assert f.dim() == 4 and f.dtype == torch.float32 and f.is_contiguous() and f.shape[3] == C and \
+            f.shape[0] == N, "level gradients must be contiguous fp32 NHWC tensors with the same N and C"
+        assert f.device == dev
+    src = (_l.RoiGradSource * len(sources))()
+    keep = []           # contiguous copies must outlive the loop: the call reads them after it
+    for s, (g, rois, coff, boff) in zip(src, sources):
+        assert g.dim() == 4 and g.shape[1] == g.shape[2] and g.shape[0] == rois.shape[0]
+        assert g.device == rois.device == dev, "gradients and level gradients must be on the RoIs' device"
+        g, rois = _f32c(g), _f32c(rois)
+        keep += [g, rois]
+        s.grad, s.rois = g.data_ptr(), rois.data_ptr()
+        s.R, s.pooled, s.ld, s.coff, s.batch_offset = g.shape[0], g.shape[1], g.shape[3], int(coff), int(boff)
+    fp = (ctypes.c_void_p * 4)(*[f.data_ptr() for f in d_feats])
+    hs = (ctypes.c_int * 4)(*[f.shape[1] for f in d_feats])
+    ws_ = (ctypes.c_int * 4)(*[f.shape[2] for f in d_feats])
+    nb = L.sb_roi_align_pyramid_backward_workspace(hs, ws_, N, C)
+    ws = workspace(nb, dev, "roi_pyramid_bwd")
+    check(L.sb_roi_align_pyramid_backward(src, len(sources), fp, hs, ws_, N, C, float(im_h), ptr(nonfinite), ptr(ws),
+                                          nb, stream_ptr()), "sb_roi_align_pyramid_backward")
+    return d_feats
+
+
 # -------------------------------------------------------- proposal layer ----
 def make_proposal_cfg(cfg_key, feat_shapes, ratios=None, scales=None, strides=None, cfg=None):
     cfg = CFG if cfg is None else cfg

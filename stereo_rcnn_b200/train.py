@@ -5,8 +5,9 @@ Host-side mirror of `_AnchorTargetLayer` (lib/model/rpn/anchor_target_layer.py:4
 stereo_rcnn.py:201-311), the multi-task sum (trainval_net.py:214-219) and `clip_gradient` (net_utils.py:37-49) over
 libstereo_b200's kernels (csrc/train_targets.cu, csrc/train_loss.cu).  No host synchronisation anywhere: counts,
 sampled indices and losses stay on the device.  rpn_gradients composes them with the engine's forward and backward
-passes into the gradients of the RPN loss for the trunk, the FPN and the RPN, and rcnn_head_gradients into the gradients
-of the R-CNN loss for the heads.
+passes into the gradients of the RPN loss for the trunk, the FPN and the RPN, rcnn_head_gradients into the gradients
+of the R-CNN loss for the heads, and loss_gradients into the gradients of the whole six-term loss for every trainable
+parameter.
 """
 import ctypes
 
@@ -251,3 +252,47 @@ def rcnn_head_gradients(engine, im_left, im_right, gt_left, gt_right, gt_merge, 
         assert uncert.numel() >= 6
         _total, d_u = multitask_loss(losses, uncert[2:6])
         return losses, hg, dpooled, d_u
+
+
+def loss_gradients(engine, im_left, im_right, gt_left, gt_right, gt_merge, gt_dim_orien, gt_kpts, keys, words,
+                   rpn_keys, dropout_words=None, uncert=None, fixed_blocks=1, grads=None, grad_scale=1.0):
+    """The whole training loss of a stereo pair (trainval_net.py:214-219) differentiated end to end on the device, each
+    step once: trunk_fpn and rpn with save_for_backward, the anchor targets for `rpn_keys` [B,A] and rpn_loss,
+    proposal_layer(..., "TRAIN") and proposal_targets for `keys` [B,R+K] / `words` [B,S], heads(save_for_backward=True,
+    dropout_words) and rcnn_loss, then rpn_backward, heads_backward, roi_align_backward of the pooled gradients into the
+    RPN's dP2..dP5, and trunk_fpn_backward(fixed_blocks).  Arguments as rpn_gradients and rcnn_head_gradients.
+    Returns (losses [6] = (rpn_loss_cls, rpn_loss_box, RCNN_loss_cls, RCNN_loss_bbox, RCNN_loss_dim_orien,
+    RCNN_loss_kpts), {state_dict name: fp32 gradient} of trainable_trunk_fpn_params(fixed_blocks) +
+    trainable_rpn_params() + trainable_rcnn_head_params(n_classes)) and, with uncert [6], d total / d uncert [6] as a
+    third item; the gradients are then those of total = sum_i losses[i] exp(-uncert[i]) + uncert[i].
+    grads / grad_scale as in the backward passes; engine.found_inf is cleared once and covers every backward pass.
+    No optimizer step, no host synchronisation."""
+    B, _, H, W = im_left.shape
+    with torch.no_grad():
+        im = torch.cat((im_left, im_right), 0).contiguous()
+        feats, saved_t = engine.trunk_fpn(im, save_for_backward=True)
+        cls_prob, bbox, shapes, saved_r, score = engine.rpn(feats, B, save_for_backward=True)
+        anchors = generate_anchors(shapes, im.device)
+        labels, tl, tr, iw, ow = anchor_targets(anchors, gt_left, gt_right, gt_merge, (H, W), rpn_keys)
+        rpn_losses, d_cls, d_box = rpn_loss(score, bbox, labels, tl, tr, iw, ow,
+                                            uncert=uncert[0:2] if uncert is not None else None)
+        from .ops import proposal_layer
+        rl, rr = proposal_layer(cls_prob, bbox, _im_info(B, H, W, im.device), "TRAIN", shapes)
+        tgt = proposal_targets(rl, rr, gt_left, gt_right, gt_dim_orien, gt_kpts, keys, words)
+        out, saved_h = engine.heads(feats, B, tgt["rois_left"].view(-1, 5), tgt["rois_right"].view(-1, 5), float(H),
+                                    save_for_backward=True, dropout_words=dropout_words)
+        # sb_rcnn_loss reads uncert[2..5] of the whole vector
+        rcnn_losses, g = rcnn_loss(out["cls_score"], out["bbox_pred"], out["dim_orien_pred"], out["kpts_pred"],
+                                   out["left_border_pred"], out["right_border_pred"], tgt, uncert=uncert)
+        grad, dp = engine.rpn_backward(saved_r, d_cls, d_box, grads=grads, grad_scale=grad_scale)
+        hg, dpooled = engine.heads_backward(saved_h, *g, grads=grads, grad_scale=grad_scale, clear_found_inf=False)
+        grad.update(hg)
+        engine.roi_align_backward(saved_h, dpooled, dp)
+        grad.update(engine.trunk_fpn_backward(saved_t, dp, fixed_blocks=fixed_blocks, grads=grads,
+                                              grad_scale=grad_scale, clear_found_inf=False))
+        losses = torch.cat((rpn_losses, rcnn_losses))
+        if uncert is None:
+            return losses, grad
+        assert uncert.numel() >= 6
+        _total, d_u = multitask_loss(losses, uncert[0:6])
+        return losses, grad, d_u
