@@ -63,9 +63,10 @@ rpn_loss_partial_kernel(const RpnArgs a, double* __restrict__ partial /*[kPartBl
         const float lab = a.labels[i];
         if (lab != -1.f) {
             const float s0 = a.cls_score[2 * i], s1 = a.cls_score[2 * i + 1];
+            // lse - s = (m - s) + log1p(exp(-|s0 - s1|)): m + log(...) - s would cancel the small loss of a
+            // well-classified anchor in fp32
             const float m = fmaxf(s0, s1);
-            const float lse = m + logf(expf(s0 - m) + expf(s1 - m));
-            ce += (double)(lse - (lab != 0.f ? s1 : s0));
+            ce += (double)((m - (lab != 0.f ? s1 : s0)) + log1pf(expf(-fabsf(s0 - s1))));
             cnt += 1.0;
         }
         const float ow = a.outside_w[i];
@@ -119,11 +120,13 @@ rpn_loss_grad_kernel(const RpnArgs a, const double* __restrict__ scal, const flo
     float d0 = 0.f, d1 = 0.f;
     if (lab != -1.f) {
         const float s0 = a.cls_score[2 * i], s1 = a.cls_score[2 * i + 1];
-        const float m = fmaxf(s0, s1);
-        const float e0 = expf(s0 - m), e1 = expf(s1 - m);
-        const float inv = 1.f / (e0 + e1);
-        d0 = (e0 * inv - (lab != 0.f ? 0.f : 1.f)) * g_cls;
-        d1 = (e1 * inv - (lab != 0.f ? 1.f : 0.f)) * g_cls;
+        // softmax of two logits: p_big = 1 / (1 + e), p_small = e / (1 + e), e = exp(-|s0 - s1|); the labelled
+        // class's p - 1 is minus the other class's p, which does not cancel when p is close to 1
+        const float e = expf(-fabsf(s0 - s1));
+        const float inv = 1.f / (1.f + e);
+        const float p0 = s0 >= s1 ? inv : e * inv, p1 = s0 >= s1 ? e * inv : inv;
+        d0 = (lab != 0.f ? p0 : -p1) * g_cls;
+        d1 = (lab != 0.f ? -p0 : p1) * g_cls;
     }
     d_cls[2 * i] = d0;
     d_cls[2 * i + 1] = d1;
@@ -175,7 +178,7 @@ __device__ __forceinline__ float row_ce(const float* __restrict__ x, int n, int 
         const float inv = 1.f / s;
         for (int j = 0; j < n; ++j) dx[j] = coef * (expf(x[j] - m) * inv - (j == cls ? 1.f : 0.f));
     }
-    return m + logf(s) - x[cls];
+    return (m - x[cls]) + logf(s);                      // no cancellation of a small loss (see rpn_loss_partial_kernel)
 }
 
 __global__ void __launch_bounds__(1024)
