@@ -495,6 +495,65 @@ size_t sb_clip_gradient_workspace(int n_tensors);
 int sb_clip_gradient(float* const* grads, const size_t* counts, int n_tensors, float clip_norm,
                      void* workspace, size_t workspace_bytes, float* norm_out, sb_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * The optimizer step and the device-side refresh of the engine's packed weights (training step, SURVEY A16).
+ *
+ * sb_sgd_step -- torch.optim.SGD.step (dampening 0, no Nesterov) over n_tensors tensors.  HOST arrays of device
+ *   pointers, element counts and per-tensor constants, passed to the kernels by value in chunks (graph-capturable):
+ *   tensor i is params[i], grads[i], moms[i] (fp32, counts[i] >= 1 elements) with weight_decay[i] >= 0 and
+ *   lr_mult[i] >= 0.  lr: fp32 [1] on the DEVICE (a captured step follows lr changes); momentum: a host float.
+ *   Per element, in this order, each operation one IEEE fp32 operation rounded to nearest (no FMA contraction):
+ *       d = g + wd * p;    m = momentum * m + d;    p = p - (lr * lr_mult) * m
+ *   A zero-initialised m gives torch's first step exactly (momentum * 0 + d = d).  skip: int32 [1] on the device (the
+ *   engine's found_inf): when *skip != 0 nothing is written and *skipped (int32 [1], device) is incremented by one --
+ *   torch.cuda.amp.GradScaler's skip-on-overflow.  SB_EINVAL before any launch for a null pointer, n_tensors < 1, a
+ *   zero count, a negative or non-finite weight_decay / lr_mult, or a non-finite momentum.
+ *
+ * sb_pack_plan / sb_pack_weights -- rewrite derived weight copies (packed, transposed, rounded, scaled) from fp32
+ *   master tensors, one launch for a whole table of targets.  Target t maps a 4-d index (i0, i1, i2, i3) < shape:
+ *       v = src[src_offset + sum_k i_k src_stride[k]]                    (strides may be negative: a tap flip)
+ *       dst[dst_offset + sum_k i_k dst_stride[k]] = T(v);  dst16[same] = (half)v when dst16 != NULL
+ *   with T one of SB_PACK_F32 (copy), SB_PACK_TF32 (round to TF32, nearest with ties away: (bits + 0x1000) & ~0x1fff,
+ *   the integer rounding of the engine's host packing), SB_PACK_F16 (fp16, round to nearest even) and
+ *   SB_PACK_SCALE_F16 (fp16 of the fp32 product v * scale[i_{scale_dim}]).  dst is fp32 for the first two, fp16 for
+ *   the others; dst16 (an fp16 twin with dst's strides) is allowed with the fp32 transforms only.  dst_stride[3] must be
+ *   1.  A target whose src_stride[3] != 1 is transposed through shared memory in tiles of up to 288 (i1, i2) rows x 32
+ *   i3 columns: the reads walk i1 fastest (put the source's fastest dimension at i1), the writes walk i3, so both are
+ *   coalesced.  sb_pack_plan validates a HOST table and fills its tile fields (tile0, tile, tiled) and *n_tiles;
+ *   sb_pack_weights re-validates the host table and launches on `targets_dev`, a device copy of it made after the plan
+ *   (upload it once, outside any capture; the launch is then graph-capturable).  SB_EINVAL before any launch for
+ *   n_targets < 1, a null table / src / dst, a non-positive extent, dst_stride[3] != 1, an unknown transform, a scale
+ *   missing or given without SB_PACK_SCALE_F16, a dst16 with an fp16 transform, an index that reaches below src or dst,
+ *   or (sb_pack_weights) tile fields that differ from the plan's.  Targets must not overlap in dst.                */
+#define SB_PACK_F32 0
+#define SB_PACK_TF32 1
+#define SB_PACK_F16 2
+#define SB_PACK_SCALE_F16 3
+
+typedef struct sb_pack_target {
+    const float* src;
+    void* dst;
+    void* dst16;               /* optional fp16 twin of dst (SB_PACK_F32 / SB_PACK_TF32 only)              */
+    const float* scale;        /* SB_PACK_SCALE_F16: per-channel scale, indexed by i_{scale_dim}           */
+    long long src_offset;      /* elements                                                                 */
+    long long dst_offset;      /* elements (dst and dst16)                                                 */
+    long long shape[4];
+    long long src_stride[4];   /* elements                                                                 */
+    long long dst_stride[4];   /* elements; dst_stride[3] == 1                                             */
+    int transform;             /* SB_PACK_*                                                                */
+    int scale_dim;             /* 0..3                                                                     */
+    long long tile0;           /* filled by sb_pack_plan: first tile (CTA) of this target                  */
+    int tile[3];               /* filled by sb_pack_plan: tile extents along i1, i2, i3                    */
+    int tiled;                 /* filled by sb_pack_plan: 1 = transposed through shared memory             */
+} sb_pack_target;
+
+int sb_sgd_step(float* const* params, float* const* grads, float* const* moms, const size_t* counts,
+                const float* weight_decay, const float* lr_mult, int n_tensors, const float* lr, float momentum,
+                const int* skip, int* skipped, sb_stream_t stream);
+int sb_pack_plan(sb_pack_target* targets, int n_targets, long long* n_tiles);
+int sb_pack_weights(const sb_pack_target* targets, const sb_pack_target* targets_dev, int n_targets,
+                    sb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,8 +6,11 @@ resnet.py:300-309 freezes every BN), left and right images run through the trunk
 batch of two, and every stage is a libstereo_b200 kernel launched on torch's current stream.
 There is no PyTorch operator on the compute path (torch only allocates device memory).
 """
+import ctypes
+
 import torch
 
+from . import lib as _lib
 from . import ops
 
 LAYERS = [3, 4, 23, 3]
@@ -118,6 +121,34 @@ class _DgradConv(object):
             w = w * scale.view(-1, 1, 1, 1)
         self.w16 = w.flip(2, 3).permute(1, 2, 3, 0).contiguous().to(torch.float16).to(device)
         self.Cin, self.Cout, self.pad = co, ci, pad
+
+
+def _numel(shape):
+    n = 1
+    for d in shape:
+        n *= int(d)
+    return n
+
+
+class _PackT(object):
+    """one sb_pack_target of engine.refresh_weights: the master tensor `name` -> dst (element strides, see
+    include/stereo_b200.h)"""
+    __slots__ = ("name", "dst", "shape", "sstr", "dstr", "transform", "src_offset", "dst_offset", "dst16", "scale")
+
+    def __init__(self, name, dst, shape, sstr, dstr, transform, src_offset=0, dst_offset=0, dst16=None, scale=None):
+        assert dst.is_contiguous() and (dst16 is None or dst16.is_contiguous())
+        self.name, self.dst, self.shape, self.sstr, self.dstr = name, dst, shape, sstr, dstr
+        self.transform, self.src_offset, self.dst_offset, self.dst16, self.scale = (transform, src_offset, dst_offset,
+                                                                                      dst16, scale)
+
+    def fill(self, t, src):
+        t.src, t.dst = src.data_ptr(), self.dst.data_ptr()
+        t.dst16 = self.dst16.data_ptr() if self.dst16 is not None else None
+        t.scale = self.scale.data_ptr() if self.scale is not None else None
+        t.src_offset, t.dst_offset = self.src_offset, self.dst_offset
+        for k in range(4):
+            t.shape[k], t.src_stride[k], t.dst_stride[k] = self.shape[k], self.sstr[k], self.dstr[k]
+        t.transform, t.scale_dim = self.transform, 3
 
 
 class PackedConv(object):
@@ -796,6 +827,118 @@ class StereoRCNNEngine(object):
                                                     (d_pooled["pooled_kpts"], s.rois_l, 0, 0)],
                                        nonfinite=self._found_inf)
         return d_feats
+
+    # ------------------------------------------------------------------ device-side refresh of the packed weights
+    def _conv_targets(self, key, name):
+        """pack targets of conv `key` from its master weight [Cout,Cin,kh,kw]: the forward's K-major copy
+        [Cout][kh][kw][Cin] (TF32-rounded fp32 plus its fp16 twin) and the data gradient's [Cin][kh][kw][Cout] fp16,
+        taps flipped, the frozen-BN scale folded in for the trunk convs"""
+        pc, bw = self.p[key], self._bwd[key]
+        co, ci, T = pc.Cout, pc.Cin, pc.kh * pc.kw
+        fw = _PackT(name, pc.w, (1, 1, 1, co * ci), (0, 0, 0, 1), (0, 0, 0, 1), self._fwd_transform, dst16=pc.w16)
+        if T > 1:       # i1 = tap, i2 = co, i3 = ci
+            fw = _PackT(name, pc.w, (1, T, co, ci), (0, 1, T * ci, T), (0, ci, T * ci, 1), self._fwd_transform,
+                        dst16=pc.w16)
+        # i1 = flipped tap t' (source tap T-1-t'), i2 = ci, i3 = co
+        scale = pc.scale if key.startswith("RCNN_layer") else None
+        dg = _PackT(name, bw.w16, (1, T, ci, co), (0, -1, T, ci * T), (0, co, T * co, 1),
+                    _lib.PACK_SCALE_F16 if scale is not None else _lib.PACK_F16, src_offset=T - 1,
+                    scale=scale)
+        return [fw, dg]
+
+    def _refresh_targets(self):
+        """{state_dict name: [_PackT]}: every derived copy of every trainable parameter, in the layouts the
+        constructor's host packing produces"""
+        L = _lib
+        self._pack_heads_backward()
+        tg = {}
+        bias = lambda name, dst: _PackT(name, dst, (1, 1, 1, dst.numel()), (0, 0, 0, 1), (0, 0, 0, 1), L.PACK_F32)
+        for key in self._bwd_src:       # trunk, FPN, RPN_Conv, RCNN_top.3, RCNN_kpts.0..10
+            if key == "rpn_heads":
+                continue
+            tg[key + ".weight"] = self._conv_targets(key, key + ".weight")
+            if self.p[key].scale is None:
+                tg[key + ".bias"] = [bias(key + ".bias", self.p[key].shift)]
+        # RPN heads: rows 0..5 / 6..23 of the fused head, columns 0..5 / 6..23 of its 64-column data-gradient copy
+        ph, bh = self.p["rpn_heads"], self._bwd["rpn_heads"]
+        for key, r0, n in (("RCNN_rpn.RPN_cls_score", 0, 6), ("RCNN_rpn.RPN_bbox_pred_left_right", 6, 18)):
+            tg[key + ".weight"] = [
+                _PackT(key + ".weight", ph.w, (1, 1, 1, n * 1024), (0, 0, 0, 1), (0, 0, 0, 1), self._fwd_transform,
+                       dst_offset=r0 * 1024, dst16=ph.w16),
+                _PackT(key + ".weight", bh.w16, (1, 1, 1024, n), (0, 0, 1, 1024), (0, 0, 64, 1), L.PACK_F16,
+                       dst_offset=r0)]
+            tg[key + ".bias"] = [_PackT(key + ".bias", ph.shift, (1, 1, 1, n), (0, 0, 0, 1), (0, 0, 0, 1), L.PACK_F32,
+                                        dst_offset=r0)]
+        # RCNN_top.0 [2048,512,7,7]: forward [co][(ph, pw, c)], data gradient [(ph, pw, c)][co]
+        pt, bt = self.p["RCNN_top.0"], self._bwd["RCNN_top.0"]
+        tg["RCNN_top.0.weight"] = [
+            _PackT("RCNN_top.0.weight", pt.w, (1, 49, 2048, 512), (0, 1, 49 * 512, 49), (0, 512, 49 * 512, 1),
+                   self._fwd_transform, dst16=pt.w16),
+            _PackT("RCNN_top.0.weight", bt.w16, (1, 49, 512, 2048), (0, 1, 49, 49 * 512), (0, 512 * 2048, 2048, 1),
+                   L.PACK_F16)]
+        tg["RCNN_top.0.bias"] = [bias("RCNN_top.0.bias", pt.shift)]
+        # deconv [Cin,Cout,2,2]: phase (a, b) forward [co][ci] = W[ci, co, a, b]; data gradient [ci][(a, b, co)]
+        name = "RCNN_kpts.12.weight"
+        tg[name] = [_PackT(name, self.deconv[a][b].w, (1, 256, 1, 256), (0, 4, 0, 1024), (0, 256, 0, 1),
+                           self._fwd_transform, src_offset=2 * a + b, dst16=self.deconv[a][b].w16)
+                    for a in range(2) for b in range(2)]
+        tg[name].append(_PackT(name, self._bwd["deconv"].w16, (1, 4, 256, 256), (0, 1, 1024, 4), (0, 256, 1024, 1),
+                               L.PACK_F16))
+        tg["RCNN_kpts.12.bias"] = [bias("RCNN_kpts.12.bias", self.deconv[a][b].shift) for a in range(2)
+                                   for b in range(2)]
+        # the fp32 linears and kpts_class: plain copies
+        for key, dst in zip(("RCNN_cls_score.weight", "RCNN_cls_score.bias", "RCNN_bbox_pred.weight",
+                             "RCNN_bbox_pred.bias", "RCNN_dim_orien_pred.weight", "RCNN_dim_orien_pred.bias",
+                             "kpts_class.weight", "kpts_class.bias"), self.fc + list(self.kpts_class)):
+            tg[key] = [bias(key, dst)]
+        return tg
+
+    @property
+    def _fwd_transform(self):
+        return _lib.PACK_F32 if self.exact else _lib.PACK_TF32
+
+    def refresh_weights(self, params):
+        """Rewrite, in place and on the device, every copy this engine holds of the parameters in `params`
+        ({state_dict name: fp32 contiguous device tensor in the reference's layout}, any subset of the trainable
+        names): the forward's packed weights (TF32-rounded fp32 and fp16), the data gradient's transposed fp16
+        copies (taps flipped, frozen-BN scale folded in), the fused RPN head and its data-gradient copy, the
+        (ph, pw, c)-ordered RCNN_top.0, the four deconv phases, biases, the linears and kpts_class.  The result is
+        bit-identical to what the constructor packs on the host from the same values.  No tensor is reallocated, so
+        CUDA graphs captured over the forward or backward stay valid.  Frozen tensors (the stem, frozen layers, the
+        BN scale and shift) are never written.
+        One launch (sb_pack_weights).  The table of a new set of (name, tensor) pairs is built and uploaded on first
+        use: make that first call outside any graph capture; later calls with the same tensors are
+        graph-capturable and do not synchronise."""
+        L = _lib
+        if not hasattr(self, "_refresh_cache"):
+            self._refresh_cache = {}
+            self._refresh_tg = self._refresh_targets()
+        for n, t in params.items():
+            if n not in self._refresh_tg:
+                raise KeyError("not a trainable parameter of this engine: %s" % n)
+            assert t.dtype == torch.float32 and t.is_contiguous() and t.device.type == self.device.type, n
+        key = tuple(sorted((n, t.data_ptr()) for n, t in params.items()))
+        ent = self._refresh_cache.get(key)
+        if ent is None:
+            items = [tp for n in sorted(params) for tp in self._refresh_tg[n]]
+            for tp in items:
+                assert params[tp.name].numel() == _numel(self._refresh_shape(tp.name)), tp.name
+            tab = (L.PackTarget * len(items))()
+            for i, tp in enumerate(items):
+                tp.fill(tab[i], params[tp.name])
+            n_tiles = ctypes.c_longlong()
+            L.check(L.load().sb_pack_plan(tab, len(items), ctypes.byref(n_tiles)), "sb_pack_plan")
+            raw = bytes(memoryview(tab).cast("B"))
+            dev = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(self.device)
+            ent = self._refresh_cache[key] = (tab, dev, len(items), [params[n] for n in sorted(params)])
+        tab, dev, n, _keep = ent
+        L.check(L.load().sb_pack_weights(tab, ops.ptr(dev), n, L.stream_ptr()), "sb_pack_weights")
+
+    def _refresh_shape(self, name):
+        if not hasattr(self, "_trainable_shapes"):
+            self._trainable_shapes = dict(trainable_trunk_fpn_params(0) + trainable_rpn_params() +
+                                          trainable_rcnn_head_params(self.n_classes))
+        return self._trainable_shapes[name]
 
     @torch.no_grad()
     def forward(self, im_left, im_right, im_info, cfg_key="TEST", keep_features=False, im_h=None,

@@ -47,6 +47,16 @@ class RoiGradSource(ctypes.Structure):
                 ("coff", c_int), ("batch_offset", c_int)]
 
 
+class PackTarget(ctypes.Structure):
+    _fields_ = [("src", c_void_p), ("dst", c_void_p), ("dst16", c_void_p), ("scale", c_void_p),
+                ("src_offset", c_ll), ("dst_offset", c_ll), ("shape", c_ll * 4), ("src_stride", c_ll * 4),
+                ("dst_stride", c_ll * 4), ("transform", c_int), ("scale_dim", c_int), ("tile0", c_ll),
+                ("tile", c_int * 3), ("tiled", c_int)]
+
+
+PACK_F32, PACK_TF32, PACK_F16, PACK_SCALE_F16 = 0, 1, 2, 3         # sb_pack_target.transform
+
+
 _SIGS = {
     "sb_version": (c_int, []),
     "sb_device_cc": (c_int, []),
@@ -151,6 +161,11 @@ _SIGS = {
     "sb_clip_gradient_workspace": (c_size_t, [c_int]),
     "sb_clip_gradient": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_size_t), c_int, c_float, c_void_p, c_size_t,
                                  c_void_p, c_void_p]),
+    # the optimizer step and the device-side weight refresh
+    "sb_sgd_step": (c_int, [ctypes.POINTER(c_void_p)] * 3 + [ctypes.POINTER(c_size_t), ctypes.POINTER(c_float),
+                            ctypes.POINTER(c_float), c_int, c_void_p, c_float, c_void_p, c_void_p, c_void_p]),
+    "sb_pack_plan": (c_int, [ctypes.POINTER(PackTarget), c_int, ctypes.POINTER(c_ll)]),
+    "sb_pack_weights": (c_int, [ctypes.POINTER(PackTarget), c_void_p, c_int, c_void_p]),
 }
 
 EXPORTS = tuple(_SIGS)

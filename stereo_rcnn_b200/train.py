@@ -151,19 +151,22 @@ def rcnn_loss(cls_score, bbox_pred, dim_orien_pred, kpts_pred, left_border_pred,
     return (losses, g) if grads else losses
 
 
-def multitask_loss(losses, uncert):
-    """trainval_net.py:214-219: losses [n], uncert [n] -> total [1], d total / d uncert [n]"""
+def multitask_loss(losses, uncert, total=None, d_uncert=None):
+    """trainval_net.py:214-219: losses [n], uncert [n] -> total [1], d total / d uncert [n] (written into `total` /
+    `d_uncert` when given)"""
     L = _l.load()
     n = losses.numel()
-    total = torch.empty(1, dtype=torch.float32, device=losses.device)
-    d_u = torch.empty(n, dtype=torch.float32, device=losses.device)
+    total = torch.empty(1, dtype=torch.float32, device=losses.device) if total is None else total
+    d_u = torch.empty(n, dtype=torch.float32, device=losses.device) if d_uncert is None else d_uncert
+    assert total.is_contiguous() and d_u.is_contiguous() and d_u.numel() == n
     check(L.sb_multitask_loss(ptr(_f32c(losses)), ptr(_f32c(uncert)), n, ptr(total), ptr(d_u), stream_ptr()),
           "sb_multitask_loss")
     return total, d_u
 
 
-def clip_gradient(grads, clip_norm):
-    """net_utils.clip_gradient over a list of fp32 gradient tensors, in place -> norm [2] (total norm, factor)"""
+def clip_gradient(grads, clip_norm, out=None):
+    """net_utils.clip_gradient over a list of fp32 gradient tensors, in place -> norm [2] (total norm, factor; written
+    into `out` when given)"""
     L = _l.load()
     n = len(grads)
     dev = grads[0].device
@@ -172,7 +175,8 @@ def clip_gradient(grads, clip_norm):
     counts = (ctypes.c_size_t * n)(*[g.numel() for g in grads])
     nbytes = L.sb_clip_gradient_workspace(n)
     ws = workspace(nbytes, dev, "clip")
-    out = torch.empty(2, dtype=torch.float32, device=dev)
+    out = torch.empty(2, dtype=torch.float32, device=dev) if out is None else out
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.numel() == 2
     check(L.sb_clip_gradient(ptrs, counts, n, float(clip_norm), ptr(ws), nbytes, ptr(out), stream_ptr()),
           "sb_clip_gradient")
     return out
@@ -255,7 +259,8 @@ def rcnn_head_gradients(engine, im_left, im_right, gt_left, gt_right, gt_merge, 
 
 
 def loss_gradients(engine, im_left, im_right, gt_left, gt_right, gt_merge, gt_dim_orien, gt_kpts, keys, words,
-                   rpn_keys, dropout_words=None, uncert=None, fixed_blocks=1, grads=None, grad_scale=1.0):
+                   rpn_keys, dropout_words=None, uncert=None, fixed_blocks=1, grads=None, grad_scale=1.0,
+                   total=None, d_uncert=None):
     """The whole training loss of a stereo pair (trainval_net.py:214-219) differentiated end to end on the device, each
     step once: trunk_fpn and rpn with save_for_backward, the anchor targets for `rpn_keys` [B,A] and rpn_loss,
     proposal_layer(..., "TRAIN") and proposal_targets for `keys` [B,R+K] / `words` [B,S], heads(save_for_backward=True,
@@ -266,7 +271,8 @@ def loss_gradients(engine, im_left, im_right, gt_left, gt_right, gt_merge, gt_di
     trainable_rpn_params() + trainable_rcnn_head_params(n_classes)) and, with uncert [6], d total / d uncert [6] as a
     third item; the gradients are then those of total = sum_i losses[i] exp(-uncert[i]) + uncert[i].
     grads / grad_scale as in the backward passes; engine.found_inf is cleared once and covers every backward pass.
-    No optimizer step, no host synchronisation."""
+    total [1] / d_uncert [6] (with uncert): fp32 device tensors that receive the multi-task total and d total /
+    d uncert in place.  No optimizer step, no host synchronisation."""
     B, _, H, W = im_left.shape
     with torch.no_grad():
         im = torch.cat((im_left, im_right), 0).contiguous()
@@ -294,5 +300,155 @@ def loss_gradients(engine, im_left, im_right, gt_left, gt_right, gt_merge, gt_di
         if uncert is None:
             return losses, grad
         assert uncert.numel() >= 6
-        _total, d_u = multitask_loss(losses, uncert[0:6])
+        _total, d_u = multitask_loss(losses, uncert[0:6], total=total, d_uncert=d_uncert)
         return losses, grad, d_u
+
+
+# ------------------------------------------------------------------------------------------------ the training step
+def _f32_ptrs(ts):
+    assert all(t.dtype == torch.float32 and t.is_contiguous() and t.is_cuda for t in ts)
+    return (ctypes.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+
+
+class _SgdArgs(object):
+    """the host arrays of one sb_sgd_step table (built once, reused by every step)"""
+
+    def __init__(self, params, grads, moms, weight_decay, lr_mult):
+        n = len(params)
+        assert len(grads) == n and len(moms) == n and len(weight_decay) == n and len(lr_mult) == n
+        for p, g, m in zip(params, grads, moms):
+            assert p.shape == g.shape == m.shape
+        self.n, self.keep = n, (list(params), list(grads), list(moms))
+        self.p, self.g, self.m = _f32_ptrs(params), _f32_ptrs(grads), _f32_ptrs(moms)
+        self.counts = (ctypes.c_size_t * n)(*[p.numel() for p in params])
+        self.wd = (ctypes.c_float * n)(*[float(w) for w in weight_decay])
+        self.lrm = (ctypes.c_float * n)(*[float(m) for m in lr_mult])
+
+    def __call__(self, lr, momentum, skip, skipped):
+        L = _l.load()
+        assert lr.dtype == torch.float32 and skip.dtype == torch.int32 and skipped.dtype == torch.int32
+        check(L.sb_sgd_step(self.p, self.g, self.m, self.counts, self.wd, self.lrm, self.n, ptr(lr), float(momentum),
+                            ptr(skip), ptr(skipped), stream_ptr()), "sb_sgd_step")
+
+
+def sgd_step(params, grads, moms, lr, momentum, weight_decay, lr_mult, skip, skipped):
+    """torch.optim.SGD.step (dampening 0, no Nesterov) over lists of fp32 device tensors, in place (sb_sgd_step):
+    per element d = g + wd p, m = momentum m + d, p = p - (lr lr_mult) m, each an fp32 operation rounded to nearest.
+    lr: fp32 [1] device tensor; weight_decay / lr_mult: one float per tensor; momentum buffers start at zero.
+    skip (int32 [1], device; e.g. engine.found_inf): when set nothing is written and skipped (int32 [1]) is
+    incremented.  No host synchronisation.  -> skipped"""
+    _SgdArgs(params, grads, moms, weight_decay, lr_mult)(lr, momentum, skip, skipped)
+    return skipped
+
+
+def trainable_names(fixed_blocks=1, n_classes=2):
+    """[(name, shape)] of every trainable tensor of the model in the order loss_gradients produces them"""
+    from . import engine as E
+    return (E.trainable_trunk_fpn_params(fixed_blocks) + E.trainable_rpn_params() +
+            E.trainable_rcnn_head_params(n_classes))
+
+
+def param_groups(names, weight_decay=1e-4, double_bias=False, bias_decay=False):
+    """trainval_net.py:158-166 per tensor -> [(lr_mult, weight_decay)]: a name containing 'bias' gets
+    lr (DOUBLE_BIAS + 1) and weight decay only with BIAS_DECAY, any other weight_decay; "uncert" gets lr and no
+    decay"""
+    out = []
+    for n in names:
+        if n == "uncert":
+            out.append((1.0, 0.0))
+        elif "bias" in n:
+            out.append((float(int(double_bias) + 1), float(bias_decay and weight_decay or 0)))
+        else:
+            out.append((1.0, float(weight_decay)))
+    return out
+
+
+def state_buckets(shapes, device, world=1, dist=None):
+    """master parameters, gradients and momentum buffers as three parallel.GradientBuckets over the same shapes:
+    one bucket plan, so view i sits at the same bucket and offset in all three.  All start at zero."""
+    from .parallel import GradientBuckets
+    return tuple(GradientBuckets(shapes, device, world=world, dist=dist) for _ in range(3))
+
+
+class Trainer(object):
+    """The training step of trainval_net.py:198-227 on the device: loss_gradients, the data-parallel gradient
+    average, clip_gradient over the model's gradients, SGD with momentum, then the engine's packed weights refreshed
+    in place from the updated masters.
+
+    Masters, gradients and momentum live in three GradientBuckets with one plan; the last view of each is `uncert`
+    [6] (trainval_net.py:155-156, initialised to -1), which is optimised with lr and no decay and is not clipped
+    (net_utils.py:37-49 walks the model's parameters only).  A step whose backward raised engine.found_inf (grad_scale
+    overflow) writes no master, momentum or packed weight and counts itself in `skipped`: GradScaler's skip, the one
+    deliberate difference from the reference.  The defaults are the reference's (config.py:22-46,
+    trainval_net.py:153-168,226).  `engine` must have been built from `state_dict` (fp16 operands); the constructor
+    uploads the refresh table and synchronises once."""
+
+    def __init__(self, engine, state_dict, fixed_blocks=1, lr=1e-3, momentum=0.9, weight_decay=1e-4,
+                 double_bias=False, bias_decay=False, clip_norm=10.0, grad_scale=1.0, world=1, dist=None):
+        self.engine, self.fixed_blocks, self.momentum = engine, int(fixed_blocks), float(momentum)
+        self.clip_norm, self.grad_scale, self.world, self.dist = float(clip_norm), float(grad_scale), int(world), dist
+        dev = engine.device
+        named = trainable_names(fixed_blocks, engine.n_classes)
+        self.names = [n for n, _ in named]
+        self.masters, self.grads, self.moms = state_buckets([s for _, s in named] + [(6,)], dev, world, dist)
+        self._sd = {k: v.detach().cpu() for k, v in state_dict.items()}
+        with torch.no_grad():
+            for n, v in zip(self.names, self.masters.grads):
+                v.copy_(self._sd[n].to(torch.float32))
+            self.masters.grads[-1].copy_(torch.full((6,), -1.0))
+        self.params = dict(zip(self.names, self.masters.grads))
+        self.uncert = self.masters.grads[-1]
+        self.grad_views = dict(zip(self.names, self.grads.grads))
+        self.groups = param_groups(self.names + ["uncert"], weight_decay, double_bias, bias_decay)
+        self._sgd = _SgdArgs(self.masters.grads, self.grads.grads, self.moms.grads, [g[1] for g in self.groups],
+                             [g[0] for g in self.groups])
+        f32 = lambda n: torch.zeros(n, dtype=torch.float32, device=dev)
+        self.lr = f32(1)
+        self.total, self.norm = f32(1), f32(2)
+        self.skipped = torch.zeros(4, dtype=torch.int32, device=dev)[:1]
+        self.set_lr(lr)
+        engine.refresh_weights(self.params)          # builds and uploads the refresh table
+        torch.cuda.synchronize(dev)
+
+    def set_lr(self, lr):
+        """the learning rate of every group, as float32(lr) of the host double (adjust_learning_rate multiplies the
+        Python value, so this follows torch's rounding); a host -> device copy: call it outside any capture.  A
+        captured step reads the new value on its next replay."""
+        self.lr_value = float(lr)
+        self.lr.copy_(torch.tensor([self.lr_value], dtype=torch.float32))
+
+    def step(self, im_left, im_right, gt_left, gt_right, gt_merge, gt_dim_orien, gt_kpts, keys, words, rpn_keys,
+             dropout_words=None):
+        """One training step on one stereo batch (arguments as loss_gradients).  Returns device tensors (losses [6],
+        total [1], [norm, clip factor] [2], skipped [1]); losses are those of the weights before the update.
+        No host synchronisation and no torch operator on the compute path (at world 1): capturable with
+        engine.GraphRunner."""
+        eng = self.engine
+        d_u = self.grads.grads[-1]
+        losses, _g, _du = loss_gradients(eng, im_left, im_right, gt_left, gt_right, gt_merge, gt_dim_orien, gt_kpts,
+                                         keys, words, rpn_keys, dropout_words=dropout_words, uncert=self.uncert,
+                                         fixed_blocks=self.fixed_blocks, grads=self.grad_views,
+                                         grad_scale=self.grad_scale, total=self.total, d_uncert=d_u)
+        if self.world > 1 and self.dist is not None:
+            self.grads.all_reduce()
+            # every rank skips the step when any rank overflowed
+            self.dist.all_reduce(eng.found_inf, op=self.dist.ReduceOp.MAX)
+        clip_gradient(self.grads.grads[:-1], self.clip_norm, out=self.norm)
+        self._sgd(self.lr, self.momentum, eng.found_inf, self.skipped)
+        eng.refresh_weights(self.params)
+        return losses, self.total, self.norm, self.skipped
+
+    def state_dict(self):
+        """host state_dict with the reference's keys: the trained masters, plus every other tensor (frozen weights,
+        BN parameters and buffers) of the state_dict the trainer was built from.  Copies to the host: a sync point."""
+        out = dict(self._sd)
+        for n, v in self.params.items():
+            out[n] = v.detach().cpu().clone()
+        return out
+
+    def checkpoint(self):
+        """what save_checkpoint stores (trainval_net.py:249-254), on the host: {"model": state_dict(), "uncert": [6],
+        "momentum": {name: momentum buffer}} (the buffers of torch.optim.SGD's state, by parameter name, "uncert"
+        included).  A sync point."""
+        mom = {n: v.detach().cpu().clone() for n, v in zip(self.names + ["uncert"], self.moms.grads)}
+        return {"model": self.state_dict(), "uncert": self.uncert.detach().cpu().clone(), "momentum": mom}
