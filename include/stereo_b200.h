@@ -554,6 +554,41 @@ int sb_pack_plan(sb_pack_target* targets, int n_targets, long long* n_tiles);
 int sb_pack_weights(const sb_pack_target* targets, const sb_pack_target* targets_dev, int n_targets,
                     sb_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * The training side of the input pipeline (SURVEY 8f-3): blobs, ground truth and random words of one step, made on
+ * the device from flags and counters that live there, so one captured graph serves every entry of a dataset.
+ *
+ * sb_prep_stereo_pair -- _get_image_blob (minibatch.py:89-131) for one pair in one launch: both frames uint8 [H,W,3],
+ *   both outputs fp32 [3,Ho,Wo] with (Ho, Wo) from sb_prep_image_size.  *flip (int32 [1], DEVICE) == 0: out_left /
+ *   out_right are sb_prep_image of left / right.  *flip != 0 (minibatch.py:116-119): out_left is sb_prep_image of the
+ *   column-mirrored RIGHT frame and out_right of the column-mirrored LEFT frame, bit for bit, without materialising
+ *   the mirrored frames.
+ * sb_train_gt -- the ground truth of a step (minibatch.py:43-85, roibatchLoader.py:72-107) for B images, one CTA per
+ *   image.  Inputs are the roidb rows of each image at a fixed capacity N <= 1024: boxes_left / boxes_right /
+ *   boxes_merge [B,N,4], gt_classes [B,N] int32, dim_orien [B,N,4] (h, w, l, theta), kpts [B,N,6], n_rows [B] int32
+ *   on the DEVICE (rows in use, clamped to [0, N] by the kernel) and words [B,N] uint32.  Rows with gt_classes == 0
+ *   are dropped; boxes and keypoints are multiplied by im_scale in fp32 (a float32 array times a Python float);
+ *   x1 = min(x1, im_width); (sin, cos) of theta are evaluated in fp64 and rounded (math.sin of a float32); a scaled
+ *   keypoint outside [0, im_width - 1] becomes -1.  The kept rows are ordered by (word, row index) ascending -- the
+ *   rule of sb_proposal_targets' samplers, in place of np.random.shuffle -- the first 30 (cfg.MAX_NUM_GT_BOXES) are
+ *   written and the rest of every output is zero: gt_left / gt_right / gt_merge [B,30,5] (x1, y1, x2, y2, class),
+ *   gt_dim_orien [B,30,5], gt_kpts [B,30,6], num_boxes [B] int32.  im_scale and im_width (the blob's width) are
+ *   those of every image of the batch.
+ * sb_random_words -- n uint32 words of Philox4x32-10: word i is element i % 4 of the block with key (seed lo, seed hi)
+ *   and counter (i / 4, stream_id, *step lo, *step hi); *step is a uint64 on the DEVICE.  The words do not depend on
+ *   the launch geometry.  Replaces the torch.randint refills of train.random_words between the replays of a step.
+ * sb_step_advance -- *step += 1 in one thread: the last node of a captured step, so every replay draws new words.
+ * SB_EINVAL before any launch for a null pointer, a non-positive size or scale, N > 1024 or n == 0.            */
+int sb_prep_stereo_pair(const uint8_t* left, const uint8_t* right, int H, int W, double scale, int rgb_input,
+                        const int* flip, float* out_left, float* out_right, sb_stream_t stream);
+int sb_train_gt(const float* boxes_left, const float* boxes_right, const float* boxes_merge, const int* gt_classes,
+                const float* dim_orien, const float* kpts, const int* n_rows, const unsigned* words, int B, int N,
+                float im_scale, int im_width, float* gt_left, float* gt_right, float* gt_merge,
+                float* gt_dim_orien, float* gt_kpts, int* num_boxes, sb_stream_t stream);
+int sb_random_words(unsigned long long seed, const unsigned long long* step, unsigned stream_id, unsigned* out,
+                    size_t n, sb_stream_t stream);
+int sb_step_advance(unsigned long long* step, sb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

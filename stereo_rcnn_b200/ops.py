@@ -781,6 +781,24 @@ def prep_image(img_u8, scale, rgb_input=False, out=None):
     return out
 
 
+def prep_stereo_pair(left_u8, right_u8, scale, flip, rgb_input=False, out=None):
+    """_get_image_blob (minibatch.py:89-131) for one pair in one launch: two uint8 [H,W,3] frames -> two fp32
+    [3,Ho,Wo] blobs.  flip: int32 [1] device tensor; when set the left blob is prep_image of the column-mirrored
+    right frame and the right blob of the mirrored left frame (minibatch.py:116-119).  out: (left, right) to write"""
+    L = _l.load()
+    assert left_u8.dtype == torch.uint8 and left_u8.dim() == 3 and left_u8.shape[2] == 3
+    assert right_u8.dtype == torch.uint8 and right_u8.shape == left_u8.shape and flip.dtype == torch.int32
+    H, W = left_u8.shape[:2]
+    ho, wo = ctypes.c_int(), ctypes.c_int()
+    check(L.sb_prep_image_size(H, W, float(scale), ctypes.byref(ho), ctypes.byref(wo)), "sb_prep_image_size")
+    if out is None:
+        out = tuple(torch.empty(3, ho.value, wo.value, dtype=torch.float32, device=left_u8.device) for _ in range(2))
+    assert all(tuple(o.shape) == (3, ho.value, wo.value) and o.dtype == torch.float32 for o in out)
+    check(L.sb_prep_stereo_pair(ptr(left_u8), ptr(right_u8), H, W, float(scale), 1 if rgb_input else 0, ptr(flip),
+                                ptr(out[0]), ptr(out[1]), stream_ptr()), "sb_prep_stereo_pair")
+    return out
+
+
 def l2_flush(buf):
     L = _l.load()
     check(L.sb_fill(ptr(buf), buf.numel(), 0.0, stream_ptr()), "sb_fill")

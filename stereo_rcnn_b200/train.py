@@ -36,6 +36,84 @@ def _words(t):
     return t
 
 
+def fill_random_words(out, seed, step, stream_id):
+    """sb_random_words: fill the int32 tensor `out` with Philox4x32-10 words that are a pure function of (seed,
+    *step, stream_id, index).  step: int64 [1] device tensor (a uint64 counter), read by the kernel, so a captured fill
+    draws new words on every replay once sb_step_advance has run.  In place of the torch.randint of random_words."""
+    assert out.dtype == torch.int32 and step.dtype == torch.int64 and step.numel() == 1
+    check(_l.load().sb_random_words(int(seed) & (2 ** 64 - 1), ptr(step), int(stream_id), ptr(out), out.numel(),
+                                    stream_ptr()), "sb_random_words")
+    return out
+
+
+def step_advance(step):
+    """sb_step_advance: *step += 1 on the device (int64 [1])"""
+    assert step.dtype == torch.int64 and step.numel() == 1
+    check(_l.load().sb_step_advance(ptr(step), stream_ptr()), "sb_step_advance")
+    return step
+
+
+GT_ROW_FIELDS = (("boxes_left", 4), ("boxes_right", 4), ("boxes_merge", 4), ("dim_orien", 4), ("kpts", 6))
+MAX_NUM_GT_BOXES = 30                                # config.py:283
+
+
+def train_gt(rows, n_rows, words, im_scale, im_width, out=None):
+    """The ground truth of a step on the device (sb_train_gt: minibatch.py:43-85 + roibatchLoader.py:72-107).
+    rows: {"boxes_left" / "boxes_right" / "boxes_merge" [B,N,4], "dim_orien" [B,N,4], "kpts" [B,N,6] fp32,
+    "gt_classes" [B,N] int32}, the roidb rows at a fixed capacity N; n_rows [B] int32 (device) rows in use;
+    words [B,N] int32 random words that order the kept rows (in place of np.random.shuffle); im_scale, im_width: the
+    scale and the width of the blob.  -> (gt_left, gt_right, gt_merge [B,30,5], gt_dim_orien [B,30,5],
+    gt_kpts [B,30,6], num_boxes [B] int32), written into `out` when given"""
+    L = _l.load()
+    B, N = rows["gt_classes"].shape
+    dev = words.device
+    assert rows["gt_classes"].dtype == torch.int32 and n_rows.dtype == torch.int32 and n_rows.numel() == B
+    assert all(rows[k].shape == (B, N, w) and rows[k].dtype == torch.float32 for k, w in GT_ROW_FIELDS)
+    assert _words(words).shape == (B, N)
+    if out is None:
+        out = tuple(torch.empty(B, MAX_NUM_GT_BOXES, w, dtype=torch.float32, device=dev) for w in (5, 5, 5, 5, 6)) + \
+            (torch.empty(B, dtype=torch.int32, device=dev),)
+    assert [tuple(o.shape[1:]) for o in out[:5]] == [(30, 5)] * 4 + [(30, 6)] and out[5].dtype == torch.int32
+    check(L.sb_train_gt(ptr(rows["boxes_left"]), ptr(rows["boxes_right"]), ptr(rows["boxes_merge"]),
+                        ptr(rows["gt_classes"]), ptr(rows["dim_orien"]), ptr(rows["kpts"]), ptr(n_rows), ptr(words),
+                        B, N, float(im_scale), int(im_width), *[ptr(o) for o in out], stream_ptr()), "sb_train_gt")
+    return out
+
+
+def _mirror_cols(a, cols_from, cols_to, width):
+    out = a.astype(np.float32).copy()
+    out[:, cols_to] = (np.float32(width) - a[:, cols_from].astype(np.float32)) - np.float32(1)
+    return out
+
+
+def append_flipped(roidb, widths):
+    """imdb.append_flipped_images (imdb.py:117-176) in numpy, once at start-up: roidb + the flip of every entry.  The
+    flip swaps the sides and mirrors the boxes (x1 = width - x2 - 1, x2 = width - x1 - 1), reflects theta (wrapped
+    into [-pi, pi] first) and takes the keypoints from `kpts_right` in the order (3, 2, 1, 0, 5, 4), all in float32.
+    The flipped entry keeps every other key of the entry and carries `kpts_right` (the mirror of `kpts`), so the
+    flip of a flip gives the first entry's geometry back.  The frames are not touched: sb_prep_stereo_pair mirrors
+    them on the device for an entry with `flipped` set."""
+    import math
+    pi, two_pi = np.float32(math.pi), np.float32(2.0 * math.pi)
+    out = list(roidb)
+    for e, w in zip(roidb, widths):
+        f = dict(e)
+        for dst, src in (("boxes_left", "boxes_right"), ("boxes_right", "boxes_left"), ("boxes_merge", "boxes_merge")):
+            f[dst] = _mirror_cols(e[src], [2, 0], [0, 2], w)
+            assert (f[dst][:, 2] >= f[dst][:, 0]).all()
+        d = e["dim_orien"].astype(np.float32).copy()
+        t = d[:, 3]
+        t = np.where(t > pi, t - two_pi, t)
+        t = np.where(t < -pi, t + two_pi, t)
+        d[:, 3] = np.where(t >= 0, pi - t, -pi - t)
+        f["dim_orien"] = d
+        f["kpts"] = _mirror_cols(e["kpts_right"], [3, 2, 1, 0, 5, 4], list(range(6)), w)
+        f["kpts_right"] = _mirror_cols(e["kpts"], [3, 2, 1, 0, 5, 4], list(range(6)), w)
+        f["flipped"] = not e.get("flipped", False)
+        out.append(f)
+    return out
+
+
 def generate_anchors(feat_shapes, device, ratios=None, scales=None, strides=None):
     """generate_anchors_all_pyramids (generate_anchors.py:157-173) on the device -> [A,4] fp32"""
     from .ops import make_proposal_cfg
@@ -384,7 +462,7 @@ class Trainer(object):
     uploads the refresh table and synchronises once."""
 
     def __init__(self, engine, state_dict, fixed_blocks=1, lr=1e-3, momentum=0.9, weight_decay=1e-4,
-                 double_bias=False, bias_decay=False, clip_norm=10.0, grad_scale=1.0, world=1, dist=None):
+                 double_bias=False, bias_decay=False, clip_norm=10.0, grad_scale=1.0, world=1, dist=None, seed=0):
         self.engine, self.fixed_blocks, self.momentum = engine, int(fixed_blocks), float(momentum)
         self.clip_norm, self.grad_scale, self.world, self.dist = float(clip_norm), float(grad_scale), int(world), dist
         dev = engine.device
@@ -406,6 +484,9 @@ class Trainer(object):
         self.lr = f32(1)
         self.total, self.norm = f32(1), f32(2)
         self.skipped = torch.zeros(4, dtype=torch.int32, device=dev)[:1]
+        # step_from_frames: the key of the step's random words and the device-side count of the steps taken
+        self.seed, self.step_count = int(seed), torch.zeros(1, dtype=torch.int64, device=dev)
+        self.epoch, self.sampler_state = 1, None     # the next epoch of fit and the state of its host generator
         self.set_lr(lr)
         engine.refresh_weights(self.params)          # builds and uploads the refresh table
         torch.cuda.synchronize(dev)
@@ -438,6 +519,29 @@ class Trainer(object):
         eng.refresh_weights(self.params)
         return losses, self.total, self.norm, self.skipped
 
+    def step_from_frames(self, inp):
+        """One training step from the buffers of a StepInputs (one stereo pair): sb_prep_stereo_pair, the random words
+        of this step (sb_random_words keyed by `seed` and the device step counter, one stream id per tensor),
+        sb_train_gt, step, then sb_step_advance -- so the next call, or the next replay of a captured call, draws new
+        words; a skipped (overflowed) step advances too.  Returns what step returns.  Outside a stream capture the
+        current stream first waits for inp.load's copies and afterwards marks the buffers as consumed; a captured call
+        holds the kernels only, and whoever replays it calls inp.ready() before and inp.release() after."""
+        capturing = torch.cuda.is_current_stream_capturing()
+        if not capturing:
+            inp.ready()
+        from .ops import prep_stereo_pair
+        prep_stereo_pair(inp.left_u8, inp.right_u8, inp.scale, inp.flip, rgb_input=inp.rgb_input,
+                         out=(inp.im_left[0], inp.im_right[0]))
+        for stream_id, t in enumerate(inp.word_tensors):
+            fill_random_words(t, self.seed, self.step_count, stream_id)
+        train_gt(inp.rows, inp.n_rows, inp.shuffle_words, inp.scale, inp.im_left.shape[3], out=inp.gt)
+        out = self.step(inp.im_left, inp.im_right, *inp.gt[:5], inp.keys, inp.words, inp.rpn_keys,
+                        dropout_words=inp.dropout_words)
+        step_advance(self.step_count)
+        if not capturing:
+            inp.release()
+        return out
+
     def state_dict(self):
         """host state_dict with the reference's keys: the trained masters, plus every other tensor (frozen weights,
         BN parameters and buffers) of the state_dict the trainer was built from.  Copies to the host: a sync point."""
@@ -449,6 +553,201 @@ class Trainer(object):
     def checkpoint(self):
         """what save_checkpoint stores (trainval_net.py:249-254), on the host: {"model": state_dict(), "uncert": [6],
         "momentum": {name: momentum buffer}} (the buffers of torch.optim.SGD's state, by parameter name, "uncert"
-        included).  A sync point."""
+        included), plus what a resumed run needs to continue as if it had not stopped: "epoch" (the next epoch of fit,
+        as the reference stores epoch + 1), "step" (the device step counter that keys the random words), "lr" and
+        "sampler_state" (fit's host generator).  A sync point."""
         mom = {n: v.detach().cpu().clone() for n, v in zip(self.names + ["uncert"], self.moms.grads)}
-        return {"model": self.state_dict(), "uncert": self.uncert.detach().cpu().clone(), "momentum": mom}
+        return {"model": self.state_dict(), "uncert": self.uncert.detach().cpu().clone(), "momentum": mom,
+                "epoch": int(self.epoch), "step": int(self.step_count.item()), "lr": self.lr_value,
+                "sampler_state": self.sampler_state}
+
+    def load_checkpoint(self, ckpt):
+        """Resume from checkpoint(): the masters, uncert, every momentum buffer (which the reference's resume,
+        trainval_net.py:170-179, leaves at zero), the step counter, the epoch and the lr, then the engine's packed
+        weights refreshed from the masters.  The frozen tensors are the engine's own: build the engine and the trainer
+        from the state_dict of the run that is resumed.  Host -> device copies: call it outside any capture."""
+        with torch.no_grad():
+            for n, v in self.params.items():
+                v.copy_(ckpt["model"][n].to(torch.float32))
+            self.uncert.copy_(ckpt["uncert"])
+            for n, v in zip(self.names + ["uncert"], self.moms.grads):
+                v.copy_(ckpt["momentum"][n])
+            self.step_count.copy_(torch.tensor([int(ckpt["step"])], dtype=torch.int64))
+        self.epoch, self.sampler_state = int(ckpt["epoch"]), ckpt.get("sampler_state")
+        self.set_lr(ckpt["lr"])
+        self.engine.refresh_weights(self.params)
+        torch.cuda.synchronize(self.engine.device)
+
+
+class StepInputs(object):
+    """The static buffers of one in-flight step_from_frames at one frame shape: the uint8 frame pair, the roidb rows
+    at capacity `max_rows` with their count, the flip flag, the two blobs, the ground truth of the step and its random
+    words.  load() fills the inputs from pinned host memory on a copy stream of its own, so with two StepInputs the
+    copy of entry k + 1 overlaps step k.  frame_hw: (H, W) of the camera frames; scale: im_scale of the blob
+    (target size / shorter side, blob.py:51); rgb_input: the frames are RGB, as image decoders give them
+    (minibatch.py:111-114), not BGR."""
+
+    def __init__(self, frame_hw, scale, device, max_rows=64, rgb_input=True, rois_per_image=None, post_nms_top_n=None):
+        from .ops import CFG as OPS_CFG
+        L = _l.load()
+        H, W = int(frame_hw[0]), int(frame_hw[1])
+        self.frame_hw, self.scale, self.rgb_input, self.device, N = (H, W), float(scale), bool(rgb_input), device, int(max_rows)
+        ho, wo = ctypes.c_int(), ctypes.c_int()
+        check(L.sb_prep_image_size(H, W, self.scale, ctypes.byref(ho), ctypes.byref(wo)), "sb_prep_image_size")
+        Ho, Wo = ho.value, wo.value
+        S = int(rois_per_image or CFG["BATCH_SIZE"])
+        R = int(post_nms_top_n or OPS_CFG["TRAIN"]["RPN_POST_NMS_TOP_N"])
+        A = len(OPS_CFG["ANCHOR_RATIOS"]) * sum((-(-Ho // s)) * (-(-Wo // s)) for s in OPS_CFG["FPN_FEAT_STRIDES"])
+        host = {"left_u8": torch.empty(H, W, 3, dtype=torch.uint8), "right_u8": torch.empty(H, W, 3, dtype=torch.uint8),
+                "gt_classes": torch.zeros(1, N, dtype=torch.int32), "n_rows": torch.zeros(1, dtype=torch.int32),
+                "flip": torch.zeros(1, dtype=torch.int32)}
+        for k, w in GT_ROW_FIELDS:
+            host[k] = torch.zeros(1, N, w, dtype=torch.float32)
+        self._host = {k: v.pin_memory() for k, v in host.items()}
+        self._dev = {k: torch.zeros_like(v, device=device) for k, v in host.items()}
+        self.left_u8, self.right_u8 = self._dev["left_u8"], self._dev["right_u8"]
+        self.n_rows, self.flip = self._dev["n_rows"], self._dev["flip"]
+        self.rows = {k: self._dev[k] for k in ("gt_classes",) + tuple(k for k, _ in GT_ROW_FIELDS)}
+        f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
+        i32 = lambda *s: torch.zeros(*s, dtype=torch.int32, device=device)
+        self.im_left, self.im_right = f(1, 3, Ho, Wo), f(1, 3, Ho, Wo)
+        self.gt = (f(1, 30, 5), f(1, 30, 5), f(1, 30, 5), f(1, 30, 5), f(1, 30, 6), i32(1))
+        self.shuffle_words, self.keys, self.words = i32(1, N), i32(1, R + MAX_NUM_GT_BOXES), i32(1, S)
+        self.rpn_keys, self.dropout_words = i32(1, A), i32(2, S, 2048)
+        # the index of a tensor here is its sb_random_words stream id
+        self.word_tensors = (self.shuffle_words, self.keys, self.words, self.rpn_keys, self.dropout_words)
+        self._copy_stream = torch.cuda.Stream(device)
+        self._copied, self._consumed = torch.cuda.Event(), torch.cuda.Event()
+
+    def load(self, entry, left, right):
+        """fill the inputs from a roidb entry and its two uint8 [H,W,3] frames (numpy arrays or tensors): a host copy
+        into pinned memory, then non_blocking copies on the copy stream, which first waits until the step that last
+        read these buffers has finished.  The host waits only for the previous load's copies out of the pinned
+        buffers."""
+        self._copied.synchronize()
+        h = self._host
+        n = int(len(entry["gt_classes"]))
+        N = h["gt_classes"].shape[1]
+        if n > N:
+            raise ValueError("%d annotation rows exceed the capacity %d of this StepInputs" % (n, N))
+        h["left_u8"].copy_(torch.as_tensor(left))
+        h["right_u8"].copy_(torch.as_tensor(right))
+        h["gt_classes"][0, :n] = torch.as_tensor(np.asarray(entry["gt_classes"], np.int32))
+        for k, _ in GT_ROW_FIELDS:
+            h[k][0, :n] = torch.as_tensor(np.asarray(entry[k], np.float32))
+        h["n_rows"][0], h["flip"][0] = n, int(bool(entry.get("flipped", False)))
+        self._copy_stream.wait_event(self._consumed)
+        with torch.cuda.stream(self._copy_stream):
+            for k, v in h.items():
+                self._dev[k].copy_(v, non_blocking=True)
+            self._copied.record(self._copy_stream)
+
+    def ready(self):
+        """the current stream waits for the copies of the last load()"""
+        torch.cuda.current_stream().wait_event(self._copied)
+
+    def release(self):
+        """the work enqueued so far on the current stream is the last reader of the loaded inputs"""
+        self._consumed.record(torch.cuda.current_stream())
+
+
+def epoch_order(n, generator):
+    """the reference sampler's order of one epoch at one pair per batch (trainval_net.py:81-101): a permutation of
+    the n entries from the host generator, no leftover"""
+    return torch.randperm(n, generator=generator).tolist()
+
+
+def lr_schedule(lr, start_epoch, epochs, lr_decay_step=5, lr_decay_gamma=0.1):
+    """[(epoch, lr)] of trainval_net.py:184-191: the lr is multiplied by gamma at the start of every epoch with
+    epoch % (lr_decay_step + 1) == 0"""
+    out = []
+    for epoch in range(start_epoch, epochs + 1):
+        if epoch % (lr_decay_step + 1) == 0:
+            lr *= lr_decay_gamma
+        out.append((epoch, lr))
+    return out
+
+
+def fit(trainer, roidb, frames, epochs, start_epoch=1, lr_decay_step=5, lr_decay_gamma=0.1, save_dir=None, log=print,
+        generator=None, target_size=600, max_rows=64, rgb_input=True):
+    """The training loop of trainval_net.py:183-258 at one stereo pair per step (minibatch.py:39-40) over
+    Trainer.step_from_frames, one CUDA graph per (frame shape, buffer set), two buffer sets per shape so that the
+    copy of the next entry overlaps the running step.
+
+    roidb: the reference's list of dicts (boxes_left, boxes_right, boxes_merge, dim_orien, kpts, gt_classes,
+    flipped; see append_flipped); frames(entry) -> (left, right) uint8 [H,W,3] arrays of the unflipped pair, decoded
+    by the caller (RGB unless rgb_input is False).  The epoch order is the reference sampler's, drawn from
+    `generator` (default: a torch.Generator seeded with trainer.seed, or continued from a loaded checkpoint); the lr
+    follows lr_schedule through trainer.set_lr.  Per step two lines go to `log` in the reference's format
+    (trainval_net.py:240-244); their numbers are copied to pinned memory behind an event and read one step late,
+    so the steady state has no device-wide synchronise.  With save_dir, trainer.checkpoint() is saved after every epoch as
+    stereo_rcnn_{epoch}_{last step}.pth (trainval_net.py:248-254).  To resume: trainer.load_checkpoint(ckpt), then
+    fit(..., start_epoch=ckpt["epoch"]).  -> [total loss of every step]"""
+    import os
+    from .engine import GraphRunner
+    dev = trainer.engine.device
+    gen = generator
+    if gen is None:
+        gen = torch.Generator()
+        if trainer.sampler_state is not None:
+            gen.set_state(trainer.sampler_state)
+        else:
+            gen.manual_seed(trainer.seed)
+    slots, runners, turn = {}, {}, {}
+    stats_host = [torch.zeros(7, dtype=torch.float32).pin_memory() for _ in range(2)]
+    stats_ev = [torch.cuda.Event() for _ in range(2)]
+    totals = []
+
+    def load(entry):
+        left, right = frames(entry)
+        hw = tuple(int(v) for v in left.shape[:2])
+        if hw not in slots:
+            slots[hw] = [StepInputs(hw, float(target_size) / float(min(hw)), dev, max_rows=max_rows,
+                                    rgb_input=rgb_input) for _ in range(2)]
+            turn[hw] = 0
+        inp = slots[hw][turn[hw]]
+        turn[hw] ^= 1
+        inp.load(entry, left, right)
+        return inp
+
+    def report(k, epoch, it, n, lr):
+        stats_ev[k].synchronize()
+        v = stats_host[k].tolist()
+        totals.append(v[6])
+        log("[epoch %2d][iter %4d/%4d] loss: %.4f, lr: %.2e" % (epoch, it, n, v[6], lr))
+        log("\t\t\trpn_cls: %.4f, rpn_box_left_right: %.4f, rcnn_cls: %.4f, rcnn_box_left_right %.4f,dim_orien %.4f, "
+            "kpts %.4f" % tuple(v[:6]))
+
+    n = len(roidb)
+    for epoch, lr in lr_schedule(trainer.lr_value, start_epoch, epochs, lr_decay_step, lr_decay_gamma):
+        if lr != trainer.lr_value:
+            trainer.set_lr(lr)
+        order = epoch_order(n, gen)
+        nxt = load(roidb[order[0]])
+        for it, idx in enumerate(order):
+            inp = nxt
+            if it + 1 < n:
+                nxt = load(roidb[order[it + 1]])
+            with torch.no_grad():
+                if id(inp) not in runners:
+                    # the first step on a buffer set runs eagerly (it creates the workspaces a capture needs); the
+                    # capture that follows launches nothing
+                    out = trainer.step_from_frames(inp)
+                    runners[id(inp)] = GraphRunner(lambda inp=inp: trainer.step_from_frames(inp), [], warmup=0)
+                else:
+                    inp.ready()
+                    out = runners[id(inp)]()
+                    inp.release()
+                k = it % 2
+                stats_host[k][:6].copy_(out[0], non_blocking=True)
+                stats_host[k][6:].copy_(out[1], non_blocking=True)
+                stats_ev[k].record()
+            if it > 0:
+                report(1 - k, epoch, it - 1, n, lr)
+        report((n - 1) % 2, epoch, n - 1, n, lr)
+        trainer.epoch, trainer.sampler_state = epoch + 1, gen.get_state()
+        if save_dir is not None:
+            name = os.path.join(save_dir, "stereo_rcnn_%d_%d.pth" % (epoch, n - 1))
+            torch.save(trainer.checkpoint(), name)
+            log("save model: %s" % name)
+    return totals
