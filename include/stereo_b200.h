@@ -123,7 +123,13 @@ int sb_roi_align_pyramid_backward(const sb_roi_grad_source* sources, int n_sourc
 /* ----------------------------------------------------- proposal layer ----
  * cls_prob [B,A,2] (column 1 = score), bbox_pred_lr [B,A,6], im_info [B,3] (device).
  * cfg: host struct (anchor pyramid + top-N / threshold constants), A = n_ratios*sum(h*w).
- * rois_left/right: [B, post_nms_top_n, 5], zero padded; fully stream-ordered.          */
+ * rois_left/right: [B, post_nms_top_n, 5], zero padded; fully stream-ordered.
+ * Scores are ranked as torch.sort(descending=True) ranks them -- every NaN above +inf, -0.0 equal to +0.0 -- with
+ * ties by ascending anchor index.  pre_nms_top_n <= 0 or >= A keeps all A anchors (K = min(pre, A) <= 16384).
+ * SB_EINVAL, before any launch, unless: every level has positive h, w, scale and stride; every ratio is finite and
+ * positive; A = n_ratios * sum(h*w) <= 2048 * 4096; post_nms_top_n >= 1; nms_thresh is finite; B >= 0; the five
+ * tensors are non-null when B > 0; the workspace is non-null and large enough.  sb_generate_anchors applies the
+ * same pyramid checks.                                                                 */
 typedef struct {
     int n_levels;             /* <= 8 */
     int shapes[8][2];         /* (h, w) of each pyramid level (rpn_shapes) */
@@ -352,7 +358,8 @@ int sb_test_decode_record(const float* rois_left, const float* rois_right, const
                           sb_stream_t stream);
 /* per-class detection NMS (test_net.py:233-259), one image: scores [R,nc], boxes [R,4nc] (decoded left
  * boxes); keeps RoIs with score[:,cls] > score_thresh, sorted by score, NMS(nms_thresh); keep[] (>= R
- * ints) receives RoI indices in kept order, num_out the count.  R <= 512.                          */
+ * ints) receives RoI indices in kept order, num_out the count.  R <= 512.  Equal scores (+0.0 and -0.0 are equal)
+ * keep ascending RoI order; a NaN score never passes the threshold.                                   */
 int sb_class_nms(const float* scores, const float* boxes, int R, int n_classes, int cls,
                  float score_thresh, float nms_thresh, int* keep, int* num_out, sb_stream_t stream);
 /* input pipeline (lib/model/utils/blob.py:44-64 prep_im_for_blob + demo.py:124-128): uint8 HWC image (BGR, or RGB

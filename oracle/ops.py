@@ -122,17 +122,26 @@ def nms_mask(dets, thresh):
 # proposal layer: lib/model/rpn/proposal_layer.py:42-145 (Q7-Q11 of SURVEY)
 # --------------------------------------------------------------------------
 def stable_order_desc(scores):
-    """total order the oracle pins: score descending, anchor index ascending"""
-    return np.argsort(-scores.astype(np.float64), kind="stable")
+    """total order the oracle pins: score descending as torch.sort(descending=True) ranks it (every NaN above +inf,
+    -0.0 equal to +0.0), ties -- NaNs included -- by ascending index"""
+    with np.errstate(invalid="ignore"):                    # signalling NaNs quieten on the cast
+        s = np.asarray(scores, np.float64).reshape(-1)
+    nan = np.isnan(s)
+    return np.lexsort((-np.where(nan, 0.0, s), ~nan))     # last key first: NaNs, then -score (stable: index)
 
 
-def proposal_layer(cls_prob, bbox_pred_lr, im_info, cfg_key, feat_shapes, return_debug=False):
-    """cls_prob [B,A,2], bbox_pred_lr [B,A,6], im_info [B,3] -> rois_left/right [B,N,5]."""
+def proposal_layer(cls_prob, bbox_pred_lr, im_info, cfg_key, feat_shapes, return_debug=False, pre_nms_top_n=None,
+                   post_nms_top_n=None, nms_thresh=None, scales=None, ratios=None, strides=None):
+    """cls_prob [B,A,2], bbox_pred_lr [B,A,6], im_info [B,3] -> rois_left/right [B,N,5].  The keyword overrides
+    replace CFG[cfg_key]'s RPN_PRE_NMS_TOP_N / RPN_POST_NMS_TOP_N / RPN_NMS_THRESH and the anchor pyramid's
+    FPN_ANCHOR_SCALES / ANCHOR_RATIOS / FPN_FEAT_STRIDES."""
     cls_prob, bbox_pred_lr, im_info = _f32(cls_prob), _f32(bbox_pred_lr), _f32(im_info)
     cfg = CFG[cfg_key]
-    pre_n, post_n, thr = cfg["RPN_PRE_NMS_TOP_N"], cfg["RPN_POST_NMS_TOP_N"], cfg["RPN_NMS_THRESH"]
+    pre_n = cfg["RPN_PRE_NMS_TOP_N"] if pre_nms_top_n is None else pre_nms_top_n
+    post_n = cfg["RPN_POST_NMS_TOP_N"] if post_nms_top_n is None else post_nms_top_n
+    thr = cfg["RPN_NMS_THRESH"] if nms_thresh is None else nms_thresh
     B, A = cls_prob.shape[:2]
-    anchors = anchors_all_pyramids(feat_shapes).astype(np.float32)
+    anchors = anchors_all_pyramids(feat_shapes, scales, ratios, strides).astype(np.float32)
     assert anchors.shape[0] == A
     out_l = np.zeros((B, post_n, 5), np.float32)
     out_r = np.zeros((B, post_n, 5), np.float32)

@@ -103,6 +103,15 @@ __device__ __forceinline__ float sb_iou(const float4 a, const float4 b) {
     return __fdiv_rn(interS, __fsub_rn(__fadd_rn(Sa, Sb), interS));
 }
 
+// Sort key of a score: a larger key ranks first, in torch.sort(descending=True)'s order -- every NaN (either sign)
+// maps to the one key just above +inf, and -0.0 to the key of +0.0.  Equal keys are ties, which callers break by
+// ascending index.
+__device__ __forceinline__ unsigned int sb_score_key(float s) {
+    if (isnan(s)) return 0xff800001u;
+    const unsigned int b = __float_as_uint(s) == 0x80000000u ? 0u : __float_as_uint(s);
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+
 // TF32 operand hygiene helpers (see sb_conv_desc.out_mode in the header)
 __device__ __forceinline__ float sb_round_tf32(float x) {
     uint32_t u;

@@ -309,11 +309,8 @@ class_nms_kernel(const float* __restrict__ scores, const float* __restrict__ box
     unsigned long long k = 0;
     if (t < R) {
         const float s = scores[(size_t)t * nc + cls];
-        if (s > score_thresh) {
-            unsigned int b = __float_as_uint(s);
-            b = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-            k = ((unsigned long long)b << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)t);
-        }
+        if (s > score_thresh)   // NaN never passes; the key of any other score is non-zero
+            k = ((unsigned long long)sb_score_key(s) << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)t);
     }
     keys[t] = k;
     __syncthreads();
@@ -514,6 +511,7 @@ extern "C" int sb_test_decode_record(const float* rois_left, const float* rois_r
 extern "C" int sb_class_nms(const float* scores, const float* boxes, int R, int n_classes, int cls,
                             float score_thresh, float nms_thresh, int* keep, int* num_out, sb_stream_t stream) {
     if (R < 0 || R > 512 || cls < 0 || cls >= n_classes || !keep || !num_out) return SB_EINVAL;
+    if (R > 0 && (!scores || !boxes)) return SB_EINVAL;
     class_nms_kernel<<<1, 512, 0, sb_cs(stream)>>>(scores, boxes, R, n_classes, cls, score_thresh, nms_thresh, keep, num_out);
     SB_LAUNCHED();
     SB_CHECK_LAUNCH();

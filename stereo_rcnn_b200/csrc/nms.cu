@@ -195,7 +195,7 @@ extern "C" int sb_nms(const float* dets, int n, float thresh, int* keep, int* nu
 
 extern "C" int sb_nms_mask(const float* dets, int n, float thresh, uint64_t* mask, sb_stream_t stream) {
     if (n <= 0) return n == 0 ? SB_OK : SB_EINVAL;
-    if (n > kTile * kMaxWords) return SB_EINVAL;
+    if (n > kTile * kMaxWords || !dets || !mask) return SB_EINVAL;
     const int cb = (n + kTile - 1) / kTile;
     cudaMemsetAsync(mask, 0, (size_t)n * cb * sizeof(uint64_t), sb_cs(stream));
     dim3 grid(cb, cb, 1);

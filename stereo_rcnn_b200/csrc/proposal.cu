@@ -16,6 +16,7 @@
 //      reduction with on-the-fly intersection and early exit at post_nms_top_n
 //   6. gather + zero padding into rois_left / rois_right
 // Memory-bound: reads scores (A*8 B) 4x from L2, deltas only for survivors.
+#include <climits>
 #include <cuda_fp16.h>
 #include "common.cuh"
 
@@ -45,10 +46,7 @@ struct SelState {
     int gt_counter;       // running slot counter for > threshold
 };
 
-__device__ __forceinline__ unsigned int ordered_key(float s) {
-    unsigned int b = __float_as_uint(s);
-    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
+// inverse of sb_score_key (common.cuh) on the keys it returns: every NaN comes back as 0x7f800001, -0.0 as +0.0
 __device__ __forceinline__ float key_to_float(unsigned int k) {
     unsigned int b = (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k;
     return __uint_as_float(b);
@@ -65,7 +63,7 @@ select_hist_kernel(const float* __restrict__ prob, int A, int pass, const SelSta
     const int nbits = pass == 2 ? 10 : 11;
     const unsigned int prefix = st->prefix;
     for (int i = blockIdx.x * 256 + threadIdx.x; i < A; i += gridDim.x * 256) {
-        unsigned int k = ordered_key(prob[2 * (size_t)i + 1]);
+        unsigned int k = sb_score_key(prob[2 * (size_t)i + 1]);
         bool match = pass == 0 || (k >> (shift + nbits)) == prefix;
         if (match) atomicAdd(&sh[(k >> shift) & ((1u << nbits) - 1)], 1);
     }
@@ -126,7 +124,7 @@ count_eq_kernel(const float* __restrict__ prob, int A, const SelState* __restric
     for (int j = 0; j < 8; ++j) {
         int i = base + j;
         if (i < A) {
-            unsigned int k = ordered_key(prob[2 * (size_t)i + 1]);
+            unsigned int k = sb_score_key(prob[2 * (size_t)i + 1]);
             ce += (k == T);
             cg += (k > T);
         }
@@ -197,7 +195,7 @@ compact_kernel(const float* __restrict__ prob, int A, const SelState* __restrict
         int i = base + j;
         keys[j] = 0;
         if (i < A) {
-            keys[j] = ordered_key(prob[2 * (size_t)i + 1]);
+            keys[j] = sb_score_key(prob[2 * (size_t)i + 1]);
             ce += (keys[j] == T);
             cg += (keys[j] > T);
         }
@@ -279,7 +277,7 @@ decode_kernel(const int* __restrict__ order, int K, const float* __restrict__ de
     const int cell = r0 / cfg.n_ratios;
     const int x = cell % cfg.width[l], y = cell / cfg.width[l];
     // generate_anchors.py:131-154: fp64 centre -/+ 0.5*size, then .type_as(scores)
-    const double cx = (double)(x * cfg.stride[l]), cy = (double)(y * cfg.stride[l]);
+    const double cx = (double)x * cfg.stride[l], cy = (double)y * cfg.stride[l];
     const double hw = 0.5 * cfg.aw[l][ratio], hh = 0.5 * cfg.ah[l][ratio];
     float4 a = make_float4((float)(cx - hw), (float)(cy - hh), (float)(cx + hw), (float)(cy + hh));
     const float* d = deltas + (size_t)idx * 6;
@@ -400,9 +398,28 @@ anchors_kernel(AnchorCfg cfg, int A, float4* __restrict__ out) {
     const int ratio = r0 % cfg.n_ratios;
     const int cell = r0 / cfg.n_ratios;
     const int x = cell % cfg.width[l], y = cell / cfg.width[l];
-    const double cx = (double)(x * cfg.stride[l]), cy = (double)(y * cfg.stride[l]);
+    const double cx = (double)x * cfg.stride[l], cy = (double)y * cfg.stride[l];
     const double hw = 0.5 * cfg.aw[l][ratio], hh = 0.5 * cfg.ah[l][ratio];
     out[idx] = make_float4((float)(cx - hw), (float)(cy - hh), (float)(cx + hw), (float)(cy + hh));
+}
+
+// the pyramid fields of cfg: 1..8 levels, each with a positive shape, scale and stride, and 1..4 finite positive
+// ratios, for at most INT_MAX anchors in all -> true when make_anchor_cfg may read them
+bool anchor_cfg_ok(const sb_proposal_cfg* pc) {
+    if (!pc || pc->n_levels < 1 || pc->n_levels > kMaxLevels || pc->n_ratios < 1 || pc->n_ratios > kMaxRatios)
+        return false;
+    for (int r = 0; r < pc->n_ratios; ++r)
+        if (!(pc->ratios[r] > 0.0) || !isfinite(pc->ratios[r])) return false;
+    long long tot = 0;
+    for (int l = 0; l < pc->n_levels; ++l) {
+        if (pc->shapes[l][0] < 1 || pc->shapes[l][1] < 1 || pc->anchor_scales[l] < 1 || pc->feat_strides[l] < 1)
+            return false;
+        const long long cells = (long long)pc->shapes[l][0] * pc->shapes[l][1];
+        if (cells > INT_MAX) return false;
+        tot += cells * pc->n_ratios;
+        if (tot > INT_MAX) return false;
+    }
+    return true;
 }
 
 int make_anchor_cfg(const sb_proposal_cfg* pc, AnchorCfg* ac) {
@@ -427,9 +444,7 @@ int make_anchor_cfg(const sb_proposal_cfg* pc, AnchorCfg* ac) {
 }  // namespace
 
 extern "C" int sb_generate_anchors(const sb_proposal_cfg* pc, int A, float* anchors, sb_stream_t stream) {
-    if (!pc || !anchors || pc->n_levels < 1 || pc->n_levels > kMaxLevels || pc->n_ratios < 1 || pc->n_ratios > kMaxRatios ||
-        (reinterpret_cast<uintptr_t>(anchors) & 15))
-        return SB_EINVAL;
+    if (!anchor_cfg_ok(pc) || !anchors || (reinterpret_cast<uintptr_t>(anchors) & 15)) return SB_EINVAL;
     AnchorCfg ac;
     if (make_anchor_cfg(pc, &ac) != A) return SB_EINVAL;
     anchors_kernel<<<sb_div_up(A, 256), 256, 0, sb_cs(stream)>>>(ac, A, reinterpret_cast<float4*>(anchors));
@@ -448,13 +463,13 @@ extern "C" int sb_proposal_layer(const float* cls_prob, const float* bbox_pred_l
                                  int B, int A, const sb_proposal_cfg* pc, float* rois_left,
                                  float* rois_right, void* workspace, size_t workspace_bytes,
                                  sb_stream_t stream) {
-    if (!pc || pc->n_levels < 1 || pc->n_levels > kMaxLevels || pc->n_ratios < 1 || pc->n_ratios > kMaxRatios)
-        return SB_EINVAL;
+    // post_nms_top_n sizes the caller's RoI buffers, so it must be positive (the reference allocates that many rows)
+    if (!anchor_cfg_ok(pc) || !isfinite(pc->nms_thresh) || pc->post_nms_top_n < 1 || B < 0) return SB_EINVAL;
+    if (B > 0 && (!cls_prob || !bbox_pred_lr || !im_info || !rois_left || !rois_right)) return SB_EINVAL;
     AnchorCfg ac;
-    const int tot = make_anchor_cfg(pc, &ac);
-    if (tot != A || B < 0) return SB_EINVAL;
+    if (make_anchor_cfg(pc, &ac) != A) return SB_EINVAL;
     const int K = (pc->pre_nms_top_n > 0 && pc->pre_nms_top_n < A) ? pc->pre_nms_top_n : A;
-    const int post_n = pc->post_nms_top_n > 0 ? pc->post_nms_top_n : K;
+    const int post_n = pc->post_nms_top_n;
     if (K > 16384 || A > kChunk * 4096) return SB_EINVAL;
     WsLayout w = ws_layout(A, K);
     if (workspace_bytes < w.total || !workspace) return SB_EINVAL;

@@ -40,7 +40,7 @@ def refk(golden_dir):
 
 
 # ------------------------------------------------------------------------ NMS
-@pytest.mark.parametrize("n", [1, 2, 63, 64, 65, 300, 1000, 6000, 12000])
+@pytest.mark.parametrize("n", [1, 2, 63, 64, 65, 127, 128, 129, 300, 1000, 4097, 6000, 12000, 16383, 16384])
 @pytest.mark.parametrize("thresh", [0.7, 0.3])
 def test_nms_bit_exact_vs_oracle(n, thresh):
     d = rand_dets(n, n)
