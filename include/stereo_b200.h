@@ -399,6 +399,23 @@ int sb_dense_align_n(const float* im_left, const float* im_right, int H, int W, 
 int sb_box_rectify(const float* boxes_all, const float* kpts_all, const float* poses_all, const float* succ,
                    const float* best_dis, const int* n, int cap, int im_h, int im_w, const double* p2,
                    const double* p3, double* final_out, sb_stream_t stream);
+/* The same three with the calibration in DEVICE memory, so that one captured CUDA graph serves every image of a
+ * split, each with its own calibration file: calib = P2 then P3, 24 row-major doubles.  Every other argument is as in
+ * the host-calibrated sibling.  The kernels read the calibration when they run; for equal calibration values the
+ * results are bit-identical to the sibling's (sb_dense_align_n_devcalib forms calib4 and the constants derived from
+ * it on the device, in the host's fp64 operations and order).  A null calib is SB_EINVAL, checked before any launch. */
+int sb_box_solve_devcalib(const float* scores, const float* boxes_left, const float* boxes_right,
+                          const float* dim_orien, const float* kpts, const int* keep, const int* num,
+                          const float* inferred, int n_classes, int cls, int im_h, int im_w, const double* calib,
+                          float eval_thresh, int cap, float* boxes_all, float* kpts_all, float* poses_all,
+                          int* src_index, int* n_out, sb_stream_t stream);
+int sb_dense_align_n_devcalib(const float* im_left, const float* im_right, int H, int W, const double* calib,
+                              double scale, const float* box_left, int box_ld, const float* keypoints,
+                              const float* poses, int pose_ld, int D_cap, const int* n_dev, float* status,
+                              float* best_dis, void* workspace, size_t workspace_bytes, sb_stream_t stream);
+int sb_box_rectify_devcalib(const float* boxes_all, const float* kpts_all, const float* poses_all, const float* succ,
+                            const float* best_dis, const int* n, int cap, int im_h, int im_w, const double* calib,
+                            double* final_out, sb_stream_t stream);
 
 /* ------------------------------------------------- record all-gather over peer memory (SURVEY 8e) ----
  * The path's only exchange: every rank's fixed-size detection record ([300, 14nc+5] fp32, ~40 KB) to every rank of

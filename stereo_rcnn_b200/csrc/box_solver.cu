@@ -62,10 +62,14 @@ struct SolveArgs {
     float eval_thresh;
 };
 
+// DEV_CALIB: the calibration is read from device memory, `calib` = P2 then P3 (24 row-major doubles), so that a
+// captured launch uses whatever was last written there; otherwise it is a.p2 / a.p3 (kernel arguments).
 // one CTA: thread i solves kept detection i, then the solved ones are compacted in order
+template <bool DEV_CALIB>
 __global__ void __launch_bounds__(kMaxDet)
 box_solve_kernel(SolveArgs a, int cap, float* __restrict__ boxes_all /*[cap,5]*/, float* __restrict__ kpts_all /*[cap,5]*/,
-                 float* __restrict__ poses_all /*[cap,8]*/, int* __restrict__ src_index /*[cap]*/, int* __restrict__ n_out) {
+                 float* __restrict__ poses_all /*[cap,8]*/, int* __restrict__ src_index /*[cap]*/, int* __restrict__ n_out,
+                 const double* __restrict__ calib /*[24], DEV_CALIB only*/) {
     __shared__ int warp_cnt[kMaxDet / 32];
     const int i = threadIdx.x;
     const int n = min(*a.num, kMaxDet);
@@ -92,7 +96,7 @@ box_solve_kernel(SolveArgs a, int cap, float* __restrict__ boxes_all /*[cap,5]*/
             const double bld[4] = {box[0], box[1], box[2], box[3]}, brd[4] = {br[0], br[1], br[2], br[3]};
             const double kpd[5] = {kp[0], kp[1], kp[2], kp[3], kp[4]};
             SbBoxProblem pb;
-            sb_box_problem(&pb, a.im_h, a.im_w, a.p2, a.p3, alpha, dim, bld, brd, kpd, 0, 0.0);
+            sb_box_problem(&pb, a.im_h, a.im_w, DEV_CALIB ? calib : a.p2, DEV_CALIB ? calib + 12 : a.p3, alpha, dim, bld, brd, kpd, 0, 0.0);
             double s[4];
             sb_box_init(pb, s);
             sb_box_lm(pb, s);
@@ -124,11 +128,13 @@ box_solve_kernel(SolveArgs a, int cap, float* __restrict__ boxes_all /*[cap,5]*/
     }
 }
 
-// after dense_align: rectified pose per solved detection (test_net.py:311-325)
+// after dense_align: rectified pose per solved detection (test_net.py:311-325); DEV_CALIB as in box_solve_kernel
+template <bool DEV_CALIB>
 __global__ void __launch_bounds__(128)
 box_rectify_kernel(const float* __restrict__ boxes_all, const float* __restrict__ kpts_all,
                    const float* __restrict__ poses_all, const float* __restrict__ succ, const float* __restrict__ dis,
-                   const int* __restrict__ n_in, int im_h, int im_w, SolveArgs a, double* __restrict__ final_out /*[cap,13]*/) {
+                   const int* __restrict__ n_in, int im_h, int im_w, SolveArgs a, double* __restrict__ final_out /*[cap,13]*/,
+                   const double* __restrict__ calib /*[24], DEV_CALIB only*/) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= *n_in) return;
     double* o = final_out + (size_t)i * 13;
@@ -141,7 +147,7 @@ box_rectify_kernel(const float* __restrict__ boxes_all, const float* __restrict_
     const double bld[4] = {b[0], b[1], b[2], b[3]};
     const double kpd[5] = {kp[0], kp[1], kp[2], kp[3], kp[4]};
     SbBoxProblem pb;
-    sb_box_problem(&pb, im_h, im_w, a.p2, a.p3, (double)ps[7], dim, bld, bld, kpd, 1, (double)dis[i]);
+    sb_box_problem(&pb, im_h, im_w, DEV_CALIB ? calib : a.p2, DEV_CALIB ? calib + 12 : a.p3, (double)ps[7], dim, bld, bld, kpd, 1, (double)dis[i]);
     double s[4];
     sb_box_init(pb, s);
     sb_box_lm(pb, s);
@@ -167,35 +173,86 @@ extern "C" int sb_infer_boundary(const float* boxes, int ld, int col_offset, con
     return SB_OK;
 }
 
-extern "C" int sb_box_solve(const float* scores, const float* boxes_left, const float* boxes_right,
+// host-calibrated (p2, p3) or device-calibrated (dcalib) launches share the argument checks and the launch
+static int box_solve_launch(const float* scores, const float* boxes_left, const float* boxes_right,
                             const float* dim_orien, const float* kpts, const int* keep, const int* num,
                             const float* inferred, int n_classes, int cls, int im_h, int im_w, const double* p2,
-                            const double* p3, float eval_thresh, int cap, float* boxes_all, float* kpts_all,
-                            float* poses_all, int* src_index, int* n_out, sb_stream_t stream) {
-    if (!scores || !boxes_left || !boxes_right || !dim_orien || !kpts || !keep || !num || !p2 || !p3 || !boxes_all ||
+                            const double* p3, const double* dcalib, float eval_thresh, int cap, float* boxes_all,
+                            float* kpts_all, float* poses_all, int* src_index, int* n_out, sb_stream_t stream) {
+    if (!scores || !boxes_left || !boxes_right || !dim_orien || !kpts || !keep || !num || !boxes_all ||
         !kpts_all || !poses_all || !src_index || !n_out || cap < 1 || cls < 0 || cls >= n_classes)
         return SB_EINVAL;
-    SolveArgs a;
+    SolveArgs a = {};
     a.scores = scores; a.boxes_l = boxes_left; a.boxes_r = boxes_right; a.dim_orien = dim_orien; a.kpts = kpts;
     a.keep = keep; a.num = num; a.inferred = inferred; a.nc = n_classes; a.cls = cls; a.im_h = im_h; a.im_w = im_w;
     a.eval_thresh = eval_thresh;
-    fill_args(&a, p2, p3);
-    box_solve_kernel<<<1, kMaxDet, 0, sb_cs(stream)>>>(a, cap, boxes_all, kpts_all, poses_all, src_index, n_out);
+    if (dcalib) {
+        box_solve_kernel<true><<<1, kMaxDet, 0, sb_cs(stream)>>>(a, cap, boxes_all, kpts_all, poses_all, src_index,
+                                                                 n_out, dcalib);
+    } else {
+        fill_args(&a, p2, p3);
+        box_solve_kernel<false><<<1, kMaxDet, 0, sb_cs(stream)>>>(a, cap, boxes_all, kpts_all, poses_all, src_index,
+                                                                  n_out, nullptr);
+    }
     SB_LAUNCHED();
     SB_CHECK_LAUNCH();
     return SB_OK;
 }
 
-extern "C" int sb_box_rectify(const float* boxes_all, const float* kpts_all, const float* poses_all, const float* succ,
+static int box_rectify_launch(const float* boxes_all, const float* kpts_all, const float* poses_all, const float* succ,
                               const float* best_dis, const int* n, int cap, int im_h, int im_w, const double* p2,
-                              const double* p3, double* final_out, sb_stream_t stream) {
-    if (!boxes_all || !kpts_all || !poses_all || !succ || !best_dis || !n || !p2 || !p3 || !final_out || cap < 1)
+                              const double* p3, const double* dcalib, double* final_out, sb_stream_t stream) {
+    if (!boxes_all || !kpts_all || !poses_all || !succ || !best_dis || !n || !final_out || cap < 1)
         return SB_EINVAL;
     SolveArgs a = {};
-    fill_args(&a, p2, p3);
-    box_rectify_kernel<<<sb_div_up(cap, 128), 128, 0, sb_cs(stream)>>>(boxes_all, kpts_all, poses_all, succ, best_dis, n,
-                                                                       im_h, im_w, a, final_out);
+    if (dcalib) {
+        box_rectify_kernel<true><<<sb_div_up(cap, 128), 128, 0, sb_cs(stream)>>>(
+            boxes_all, kpts_all, poses_all, succ, best_dis, n, im_h, im_w, a, final_out, dcalib);
+    } else {
+        fill_args(&a, p2, p3);
+        box_rectify_kernel<false><<<sb_div_up(cap, 128), 128, 0, sb_cs(stream)>>>(
+            boxes_all, kpts_all, poses_all, succ, best_dis, n, im_h, im_w, a, final_out, nullptr);
+    }
     SB_LAUNCHED();
     SB_CHECK_LAUNCH();
     return SB_OK;
+}
+
+extern "C" int sb_box_solve(const float* scores, const float* boxes_left, const float* boxes_right,
+                            const float* dim_orien, const float* kpts, const int* keep, const int* num,
+                            const float* inferred, int n_classes, int cls, int im_h, int im_w, const double* p2,
+                            const double* p3, float eval_thresh, int cap, float* boxes_all, float* kpts_all,
+                            float* poses_all, int* src_index, int* n_out, sb_stream_t stream) {
+    if (!p2 || !p3) return SB_EINVAL;
+    return box_solve_launch(scores, boxes_left, boxes_right, dim_orien, kpts, keep, num, inferred, n_classes, cls, im_h,
+                            im_w, p2, p3, nullptr, eval_thresh, cap, boxes_all, kpts_all, poses_all, src_index, n_out,
+                            stream);
+}
+
+extern "C" int sb_box_solve_devcalib(const float* scores, const float* boxes_left, const float* boxes_right,
+                                     const float* dim_orien, const float* kpts, const int* keep, const int* num,
+                                     const float* inferred, int n_classes, int cls, int im_h, int im_w,
+                                     const double* calib, float eval_thresh, int cap, float* boxes_all,
+                                     float* kpts_all, float* poses_all, int* src_index, int* n_out,
+                                     sb_stream_t stream) {
+    if (!calib) return SB_EINVAL;
+    return box_solve_launch(scores, boxes_left, boxes_right, dim_orien, kpts, keep, num, inferred, n_classes, cls, im_h,
+                            im_w, nullptr, nullptr, calib, eval_thresh, cap, boxes_all, kpts_all, poses_all, src_index,
+                            n_out, stream);
+}
+
+extern "C" int sb_box_rectify(const float* boxes_all, const float* kpts_all, const float* poses_all, const float* succ,
+                              const float* best_dis, const int* n, int cap, int im_h, int im_w, const double* p2,
+                              const double* p3, double* final_out, sb_stream_t stream) {
+    if (!p2 || !p3) return SB_EINVAL;
+    return box_rectify_launch(boxes_all, kpts_all, poses_all, succ, best_dis, n, cap, im_h, im_w, p2, p3, nullptr,
+                              final_out, stream);
+}
+
+extern "C" int sb_box_rectify_devcalib(const float* boxes_all, const float* kpts_all, const float* poses_all,
+                                       const float* succ, const float* best_dis, const int* n, int cap, int im_h,
+                                       int im_w, const double* calib, double* final_out, sb_stream_t stream) {
+    if (!calib) return SB_EINVAL;
+    return box_rectify_launch(boxes_all, kpts_all, poses_all, succ, best_dis, n, cap, im_h, im_w, nullptr, nullptr,
+                              calib, final_out, stream);
 }

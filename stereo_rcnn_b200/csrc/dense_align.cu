@@ -64,6 +64,22 @@ struct Consts {
     UpGeom ug;
 };
 
+// dense_align_impl's calibration constants, formed on the device from 24 doubles in device memory (P2 then P3,
+// row-major): calib4 = [p2[0], p2[2], p2[6], p2[3] - p3[3]] and then the host's fp64 operations in the host's order,
+// each rounded explicitly so that nothing is contracted -- the same values the host puts in a launch's Consts.
+__device__ __forceinline__ void calib_consts(Consts* k, const double* __restrict__ calib, double scale) {
+    const double c0 = calib[0], c1 = calib[2], c2 = calib[6], c3 = __dsub_rn(calib[3], calib[15]);
+    const double s2 = __dmul_rn(scale, 2.0);
+    const double fd = __dmul_rn(c0, s2);
+    const double bld = __ddiv_rn(__dmul_rn(c3, s2), fd);
+    k->s2f = __double2float_rn(s2);
+    k->f32 = __double2float_rn(fd);
+    k->bl32 = __double2float_rn(bld);
+    k->fb32 = __double2float_rn(__dmul_rn(fd, bld));
+    k->cx32 = __double2float_rn(__dmul_rn(c1, s2));
+    k->cy32 = __double2float_rn(__dmul_rn(c2, s2));
+}
+
 struct RoiCtx {
     float T[3];
     float c, s;
@@ -491,14 +507,17 @@ __device__ __forceinline__ int argmin_partials(const float* __restrict__ part, i
     return bi;
 }
 
-// grid (D, S): S row slices per RoI so that a few dozen RoIs still fill the machine; dynamic smem = the strip
-template <int STAGE>
+// grid (D, S): S row slices per RoI so that a few dozen RoIs still fill the machine; dynamic smem = the strip.
+// DEV_CALIB: the calibration constants of `k0` are formed in the prologue from `calib` [24] (device memory) and
+// `scale`; otherwise `k0` holds them and the last two arguments are unused.
+template <int STAGE, bool DEV_CALIB>
 __global__ void __launch_bounds__(256)
 dense_stage_kernel(const float* __restrict__ imL, const float* __restrict__ imR, const float4* __restrict__ upL,
-                   const float4* __restrict__ upR, Consts k,
+                   const float4* __restrict__ upR, Consts k0,
                    const float* __restrict__ box_left, const float* __restrict__ keypoints,
                    const float* __restrict__ poses, int box_ld, int pose_ld, float* __restrict__ part0 /*[D][S][51]*/,
-                   float* __restrict__ part1 /*[D][S][21]*/, const int* __restrict__ n_dev) {
+                   float* __restrict__ part1 /*[D][S][21]*/, const int* __restrict__ n_dev,
+                   const double* __restrict__ calib, double scale) {
     extern __shared__ float4 strip[];        // [2][kStripMax]
     if (n_dev && (int)blockIdx.x >= *n_dev) return;      // device-side RoI count (the solver's output): CTA-uniform
     __shared__ RoiCtx g;
@@ -506,8 +525,13 @@ dense_stage_kernel(const float* __restrict__ imL, const float* __restrict__ imR,
     __shared__ float red[8 * 51];
     __shared__ float best_depth;
     __shared__ int best_idx;
+    __shared__ Consts k_dev;
+    const Consts& k = DEV_CALIB ? k_dev : k0;            // k_dev is written by thread 0 before the first barrier
     const int i = blockIdx.x, S = gridDim.y;
-    if (threadIdx.x == 0) setup_roi(box_left + (size_t)box_ld * i, keypoints + 5 * i, poses + (size_t)pose_ld * i, k, &g);
+    if (threadIdx.x == 0) {
+        if (DEV_CALIB) { k_dev = k0; calib_consts(&k_dev, calib, scale); }
+        setup_roi(box_left + (size_t)box_ld * i, keypoints + 5 * i, poses + (size_t)pose_ld * i, k, &g);
+    }
     if (STAGE == 1 && threadIdx.x >= 32 && threadIdx.x < 64) {      // warp 1, concurrently with the box setup
         const int bi = argmin_partials(part0 + (size_t)i * S * 51, S, 50, 51, nullptr);
         if (threadIdx.x == 32) best_idx = bi;
@@ -530,13 +554,21 @@ dense_stage_kernel(const float* __restrict__ imL, const float* __restrict__ imR,
 }
 
 // one CTA, one warp per RoI: argmins, outputs, and the reference's "no valid pixel anywhere -> dis_init" early-out
+// (DEV_CALIB as in dense_stage_kernel)
+template <bool DEV_CALIB>
 __global__ void __launch_bounds__(256)
-dense_final_kernel(Consts k, const float* __restrict__ poses, int pose_ld, const float* __restrict__ part0,
+dense_final_kernel(Consts k0, const float* __restrict__ poses, int pose_ld, const float* __restrict__ part0,
                    const float* __restrict__ part1, int D, int S, float* __restrict__ status,
-                   float* __restrict__ best_dis, const int* __restrict__ n_dev) {
+                   float* __restrict__ best_dis, const int* __restrict__ n_dev, const double* __restrict__ calib,
+                   double scale) {
     __shared__ int any_valid;
+    __shared__ Consts k_dev;
+    const Consts& k = DEV_CALIB ? k_dev : k0;
     if (n_dev) D = min(D, *n_dev);
-    if (threadIdx.x == 0) any_valid = 0;
+    if (threadIdx.x == 0) {
+        any_valid = 0;
+        if (DEV_CALIB) { k_dev = k0; calib_consts(&k_dev, calib, scale); }
+    }
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
     for (int i = warp; i < D; i += nw) {
@@ -584,17 +616,20 @@ DaLayout da_layout(int H, int W, int D) {
 
 extern "C" size_t sb_dense_align_workspace_bytes(int H, int W, int D) { return da_layout(H, W, D).total; }
 
+// exactly one of calib4 (host, [4]) and dcalib (device, [24]) is non-null
 static int dense_align_impl(const float* im_left, const float* im_right, int H, int W, const double* calib4,
-                            double scale, const float* box_left, int box_ld, const float* keypoints, const float* poses,
-                            int pose_ld, int D, const int* n_dev, float* status, float* best_dis, void* workspace,
-                            size_t workspace_bytes, sb_stream_t stream);
+                            const double* dcalib, double scale, const float* box_left, int box_ld,
+                            const float* keypoints, const float* poses, int pose_ld, int D, const int* n_dev,
+                            float* status, float* best_dis, void* workspace, size_t workspace_bytes,
+                            sb_stream_t stream);
 
 extern "C" int sb_dense_align(const float* im_left, const float* im_right, int H, int W, const double* calib4,
                               double scale, const float* box_left, const float* keypoints, const float* poses,
                               int D, float* status, float* best_dis, void* workspace, size_t workspace_bytes,
                               sb_stream_t stream) {
-    return dense_align_impl(im_left, im_right, H, W, calib4, scale, box_left, 4, keypoints, poses, 7, D, nullptr, status,
-                            best_dis, workspace, workspace_bytes, stream);
+    if (D != 0 && !calib4) return SB_EINVAL;
+    return dense_align_impl(im_left, im_right, H, W, calib4, nullptr, scale, box_left, 4, keypoints, poses, 7, D, nullptr,
+                            status, best_dis, workspace, workspace_bytes, stream);
 }
 
 // D_cap rows are launched; rows >= *n_dev (a device-resident count, e.g. sb_box_solve's n_out) do no work and get no
@@ -605,16 +640,30 @@ extern "C" int sb_dense_align_n(const float* im_left, const float* im_right, int
                                 const float* poses, int pose_ld, int D_cap, const int* n_dev, float* status,
                                 float* best_dis, void* workspace, size_t workspace_bytes, sb_stream_t stream) {
     if (!n_dev || box_ld < 4 || pose_ld < 7) return SB_EINVAL;
-    return dense_align_impl(im_left, im_right, H, W, calib4, scale, box_left, box_ld, keypoints, poses, pose_ld, D_cap,
-                            n_dev, status, best_dis, workspace, workspace_bytes, stream);
+    if (D_cap != 0 && !calib4) return SB_EINVAL;
+    return dense_align_impl(im_left, im_right, H, W, calib4, nullptr, scale, box_left, box_ld, keypoints, poses, pose_ld,
+                            D_cap, n_dev, status, best_dis, workspace, workspace_bytes, stream);
+}
+
+// sb_dense_align_n with the calibration read on the device: calib = P2 then P3, 24 row-major doubles in device
+// memory.  The constants the host forms from calib4 are formed in each CTA's prologue, in the same fp64 operations.
+extern "C" int sb_dense_align_n_devcalib(const float* im_left, const float* im_right, int H, int W,
+                                         const double* calib, double scale, const float* box_left, int box_ld,
+                                         const float* keypoints, const float* poses, int pose_ld, int D_cap,
+                                         const int* n_dev, float* status, float* best_dis, void* workspace,
+                                         size_t workspace_bytes, sb_stream_t stream) {
+    if (!calib || !n_dev || box_ld < 4 || pose_ld < 7) return SB_EINVAL;
+    return dense_align_impl(im_left, im_right, H, W, nullptr, calib, scale, box_left, box_ld, keypoints, poses, pose_ld,
+                            D_cap, n_dev, status, best_dis, workspace, workspace_bytes, stream);
 }
 
 static int dense_align_impl(const float* im_left, const float* im_right, int H, int W, const double* calib4,
-                            double scale, const float* box_left, int box_ld, const float* keypoints, const float* poses,
-                            int pose_ld, int D, const int* n_dev, float* status, float* best_dis, void* workspace,
-                            size_t workspace_bytes, sb_stream_t stream) {
+                            const double* dcalib, double scale, const float* box_left, int box_ld,
+                            const float* keypoints, const float* poses, int pose_ld, int D, const int* n_dev,
+                            float* status, float* best_dis, void* workspace, size_t workspace_bytes,
+                            sb_stream_t stream) {
     if (D == 0) return SB_OK;
-    if (D < 0 || H < 2 || W < 2 || !im_left || !im_right || !calib4 || !workspace) return SB_EINVAL;
+    if (D < 0 || H < 2 || W < 2 || !im_left || !im_right || !workspace) return SB_EINVAL;
     DaLayout l = da_layout(H, W, D);
     if (workspace_bytes < l.total) return SB_EINVAL;
     char* ws = (char*)workspace;
@@ -624,17 +673,20 @@ static int dense_align_impl(const float* im_left, const float* im_right, int H, 
     const bool materialise = D > kStripMaxD;
     float4* upL = materialise ? (float4*)(ws + l.upL) : nullptr;
     float4* upR = materialise ? (float4*)(ws + l.upR) : nullptr;
-    // dense_align.py:255-266 (python floats = doubles, cast to fp32 where they meet a tensor)
-    const double s2 = scale * 2.0;
-    const double fd = calib4[0] * s2;
-    const double bld = calib4[3] * s2 / fd;
-    Consts k;
-    k.s2f = (float)s2;
-    k.f32 = (float)fd;
-    k.bl32 = (float)bld;
-    k.fb32 = (float)(fd * bld);
-    k.cx32 = (float)(calib4[1] * s2);
-    k.cy32 = (float)(calib4[2] * s2);
+    // dense_align.py:255-266 (python floats = doubles, cast to fp32 where they meet a tensor); with dcalib the
+    // kernels form these six from device memory (calib_consts) and they stay zero here
+    Consts k = {};
+    if (calib4) {
+        const double s2 = scale * 2.0;
+        const double fd = calib4[0] * s2;
+        const double bld = calib4[3] * s2 / fd;
+        k.s2f = (float)s2;
+        k.f32 = (float)fd;
+        k.bl32 = (float)bld;
+        k.fb32 = (float)(fd * bld);
+        k.cx32 = (float)(calib4[1] * s2);
+        k.cy32 = (float)(calib4[2] * s2);
+    }
     k.FH = 2 * H;
     k.FW = 2 * W;
     k.fw2 = (float)(((double)k.FW - 1.0) / 2.0);
@@ -646,9 +698,12 @@ static int dense_align_impl(const float* im_left, const float* im_right, int H, 
     constexpr size_t kStripBytes = (size_t)2 * kStripMax * sizeof(float4);
     static bool attr_done[kSbMaxDevices] = {false};
     if (!attr_done[sb_cur_device()]) {
-        cudaError_t e = cudaFuncSetAttribute(dense_stage_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStripBytes);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(dense_stage_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStripBytes);
-        if (e != cudaSuccess) return (int)e;
+        const void* stage[4] = {(const void*)dense_stage_kernel<0, false>, (const void*)dense_stage_kernel<1, false>,
+                                (const void*)dense_stage_kernel<0, true>, (const void*)dense_stage_kernel<1, true>};
+        for (const void* f : stage) {
+            const cudaError_t e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStripBytes);
+            if (e != cudaSuccess) return (int)e;
+        }
         attr_done[sb_cur_device()] = true;
     }
     int S = (materialise ? 296 : 592) / D;     // strip kernel: ~4 CTAs per SM (its per-row phases are latency bound)
@@ -659,12 +714,22 @@ static int dense_align_impl(const float* im_left, const float* im_right, int H, 
         SB_CHECK_LAUNCH();
     }
     S = S < 1 ? 1 : (S > kMaxSlices ? kMaxSlices : S);
-    dense_stage_kernel<0><<<dim3(D, S), 256, materialise ? 0 : kStripBytes, st>>>(im_left, im_right, upL, upR, k, box_left, keypoints, poses, box_ld, pose_ld, part0, part1, n_dev);
-    SB_LAUNCHED();
-    dense_stage_kernel<1><<<dim3(D, S), 256, materialise ? 0 : kStripBytes, st>>>(im_left, im_right, upL, upR, k, box_left, keypoints, poses, box_ld, pose_ld, part0, part1, n_dev);
-    SB_LAUNCHED();
-    dense_final_kernel<<<1, 256, 0, st>>>(k, poses, pose_ld, part0, part1, D, S, status, best_dis, n_dev);
-    SB_LAUNCHED();
+    const size_t smem = materialise ? 0 : kStripBytes;
+    if (dcalib) {
+        dense_stage_kernel<0, true><<<dim3(D, S), 256, smem, st>>>(im_left, im_right, upL, upR, k, box_left, keypoints, poses, box_ld, pose_ld, part0, part1, n_dev, dcalib, scale);
+        SB_LAUNCHED();
+        dense_stage_kernel<1, true><<<dim3(D, S), 256, smem, st>>>(im_left, im_right, upL, upR, k, box_left, keypoints, poses, box_ld, pose_ld, part0, part1, n_dev, dcalib, scale);
+        SB_LAUNCHED();
+        dense_final_kernel<true><<<1, 256, 0, st>>>(k, poses, pose_ld, part0, part1, D, S, status, best_dis, n_dev, dcalib, scale);
+        SB_LAUNCHED();
+    } else {
+        dense_stage_kernel<0, false><<<dim3(D, S), 256, smem, st>>>(im_left, im_right, upL, upR, k, box_left, keypoints, poses, box_ld, pose_ld, part0, part1, n_dev, nullptr, 0.0);
+        SB_LAUNCHED();
+        dense_stage_kernel<1, false><<<dim3(D, S), 256, smem, st>>>(im_left, im_right, upL, upR, k, box_left, keypoints, poses, box_ld, pose_ld, part0, part1, n_dev, nullptr, 0.0);
+        SB_LAUNCHED();
+        dense_final_kernel<false><<<1, 256, 0, st>>>(k, poses, pose_ld, part0, part1, D, S, status, best_dis, n_dev, nullptr, 0.0);
+        SB_LAUNCHED();
+    }
     SB_CHECK_LAUNCH();
     return SB_OK;
 }

@@ -97,6 +97,13 @@ _SIGS = {
                              ctypes.POINTER(c_double), c_float, c_int] + [c_void_p] * 5 + [c_void_p]),
     "sb_box_rectify": (c_int, [c_void_p] * 6 + [c_int, c_int, c_int, ctypes.POINTER(c_double),
                                ctypes.POINTER(c_double), c_void_p, c_void_p]),
+    # the same three with the calibration (P2 then P3, 24 doubles) in device memory
+    "sb_box_solve_devcalib": (c_int, [c_void_p] * 8 + [c_int, c_int, c_int, c_int, c_void_p, c_float, c_int] +
+                              [c_void_p] * 5 + [c_void_p]),
+    "sb_dense_align_n_devcalib": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_double, c_void_p, c_int,
+                                          c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                          c_size_t, c_void_p]),
+    "sb_box_rectify_devcalib": (c_int, [c_void_p] * 6 + [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "sb_conv2d_simt": (c_int, [ctypes.POINTER(ConvDesc), c_void_p]),
     "sb_conv2d_tc": (c_int, [ctypes.POINTER(ConvDesc), c_void_p]),
     "sb_conv2d_tc_supported": (c_int, [ctypes.POINTER(ConvDesc)]),

@@ -3,6 +3,7 @@
 Every function launches hand-written sm_90a kernels from libstereo_b200.so on
 torch's current stream; nothing here computes on the host and nothing falls back.
 """
+import collections
 import contextlib
 import ctypes
 import threading
@@ -272,9 +273,25 @@ def dense_align(calib4, scale, im_left, im_right, box_left, keypoints, poses):
     return status, best
 
 
+def device_calib(p2, p3, device):
+    """the device calibration of the *_devcalib entry points: P2 then P3, row-major, fp64 [24] on `device`"""
+    c = np.concatenate([np.asarray(p2, np.float64).reshape(12), np.asarray(p3, np.float64).reshape(12)])
+    return torch.from_numpy(c).to(device)
+
+
+def _devcalib(c):
+    """c if it is a device calibration (a CUDA fp64 tensor [24]), else None"""
+    if not torch.is_tensor(c):
+        return None
+    assert c.is_cuda and c.dtype == torch.float64 and c.numel() == 24 and c.is_contiguous(), \
+        "a device calibration is a contiguous CUDA fp64 tensor [24] (P2 then P3, row-major)"
+    return c
+
+
 def dense_align_n(calib4, scale, im_left, im_right, boxes_all, keypoints, poses_all, n_dev):
     """align_parallel on device-resident solver outputs: boxes_all [cap,>=4], keypoints [cap,5], poses_all [cap,>=7],
-    n_dev int32 [1] (how many rows are live) -> status [cap], best_dis [cap]; rows >= n are left at zero"""
+    n_dev int32 [1] (how many rows are live) -> status [cap], best_dis [cap]; rows >= n are left at zero.
+    calib4: calib_vec(p2, p3) on the host, or a device calibration [24] (device_calib), read when the kernels run"""
     L = _l.load()
     iml = _f32c(im_left).reshape(3, *im_left.shape[-2:])
     imr = _f32c(im_right).reshape(3, *im_right.shape[-2:])
@@ -285,6 +302,13 @@ def dense_align_n(calib4, scale, im_left, im_right, boxes_all, keypoints, poses_
     best = torch.zeros(cap, dtype=torch.float32, device=dev)
     nb = L.sb_dense_align_workspace_bytes(H, W, cap)
     ws = workspace(nb, dev, "dense_align")
+    dc = _devcalib(calib4)
+    if dc is not None:
+        check(L.sb_dense_align_n_devcalib(ptr(iml), ptr(imr), H, W, ptr(dc), float(scale), ptr(_f32c(boxes_all)),
+                                          boxes_all.shape[1], ptr(_f32c(keypoints)), ptr(_f32c(poses_all)),
+                                          poses_all.shape[1], cap, ptr(n_dev), ptr(status), ptr(best), ptr(ws), nb,
+                                          stream_ptr()), "sb_dense_align_n_devcalib")
+        return status, best
     c4 = (ctypes.c_double * 4)(*[float(v) for v in calib4])
     check(L.sb_dense_align_n(ptr(iml), ptr(imr), H, W, c4, float(scale), ptr(_f32c(boxes_all)), boxes_all.shape[1],
                              ptr(_f32c(keypoints)), ptr(_f32c(poses_all)), poses_all.shape[1], cap, ptr(n_dev),
@@ -310,7 +334,8 @@ def infer_boundary(boxes, keep, num, im_w, col_offset=0):
 def box_solve(scores, boxes_left, boxes_right, dim_orien, kpts, keep, num, im_hw, p2, p3, cls=1, eval_thresh=0.05,
               inferred=None, cap=None):
     """test_net.py:263-303 on the device: border fix-up + solve_x_y_z_theta_from_kpt per kept detection, solved ones
-    appended in order -> boxes_all [cap,5], kpts_all [cap,5], poses_all [cap,8], src_index [cap], n [1] (device)"""
+    appended in order -> boxes_all [cap,5], kpts_all [cap,5], poses_all [cap,8], src_index [cap], n [1] (device).
+    p2, p3: host 3x4 matrices, or p2 a device calibration [24] (device_calib) and p3 None"""
     L = _l.load()
     R, nc = scores.shape
     cap = R if cap is None else int(cap)
@@ -320,6 +345,15 @@ def box_solve(scores, boxes_left, boxes_right, dim_orien, kpts, keep, num, im_hw
     poses_all = torch.zeros(cap, 8, dtype=torch.float32, device=dev)
     src = torch.zeros(cap, dtype=torch.int32, device=dev)
     n = torch.zeros(1, dtype=torch.int32, device=dev)
+    dc = _devcalib(p2)
+    if dc is not None:
+        assert p3 is None, "with a device calibration p3 is None"
+        check(L.sb_box_solve_devcalib(ptr(_f32c(scores)), ptr(_f32c(boxes_left)), ptr(_f32c(boxes_right)),
+                                      ptr(_f32c(dim_orien)), ptr(_f32c(kpts)), ptr(keep), ptr(num), ptr(inferred), nc,
+                                      int(cls), int(im_hw[0]), int(im_hw[1]), ptr(dc), float(eval_thresh), cap,
+                                      ptr(boxes_all), ptr(kpts_all), ptr(poses_all), ptr(src), ptr(n), stream_ptr()),
+              "sb_box_solve_devcalib")
+        return boxes_all, kpts_all, poses_all, src, n
     check(L.sb_box_solve(ptr(_f32c(scores)), ptr(_f32c(boxes_left)), ptr(_f32c(boxes_right)), ptr(_f32c(dim_orien)),
                          ptr(_f32c(kpts)), ptr(keep), ptr(num), ptr(inferred), nc, int(cls), int(im_hw[0]),
                          int(im_hw[1]), _p34(p2), _p34(p3), float(eval_thresh), cap, ptr(boxes_all), ptr(kpts_all),
@@ -329,13 +363,44 @@ def box_solve(scores, boxes_left, boxes_right, dim_orien, kpts, keep, num, im_hw
 
 def box_rectify(boxes_all, kpts_all, poses_all, succ, best_dis, n, im_hw, p2, p3):
     """test_net.py:311-325: solve_x_y_theta_from_kpt with the aligned disparity -> final [cap,13] float64
-    (valid, score, box_left 4, x, y, z, w, h, l, theta)"""
+    (valid, score, box_left 4, x, y, z, w, h, l, theta).  p2, p3 as in box_solve"""
     L = _l.load()
     cap = boxes_all.shape[0]
     out = torch.zeros(cap, 13, dtype=torch.float64, device=boxes_all.device)
+    dc = _devcalib(p2)
+    if dc is not None:
+        assert p3 is None, "with a device calibration p3 is None"
+        check(L.sb_box_rectify_devcalib(ptr(boxes_all), ptr(kpts_all), ptr(poses_all), ptr(succ), ptr(best_dis), ptr(n),
+                                        cap, int(im_hw[0]), int(im_hw[1]), ptr(dc), ptr(out), stream_ptr()),
+              "sb_box_rectify_devcalib")
+        return out
     check(L.sb_box_rectify(ptr(boxes_all), ptr(kpts_all), ptr(poses_all), ptr(succ), ptr(best_dis), ptr(n), cap,
                            int(im_hw[0]), int(im_hw[1]), _p34(p2), _p34(p3), ptr(out), stream_ptr()), "sb_box_rectify")
     return out
+
+
+Calibration = collections.namedtuple("Calibration", "p0 p1 p2 p3 t_cam2_cam0_x")
+
+
+def read_calibration(path_or_text):
+    """kitti_utils.read_obj_calibration (kitti_utils.py:97-159) for what the test loop reads: a KITTI calib/*.txt, given
+    as a path or as its text (anything with a line break) -> Calibration(p0, p1, p2, p3 [3,4] float64,
+    t_cam2_cam0_x), t_cam2_cam0_x = (p2[0,3] - p0[0,3]) / p2[0,0] (what write_detection_results subtracts from x).
+    Host side: parsing text is not device work."""
+    text = path_or_text
+    if "\n" not in text:
+        with open(path_or_text) as f:
+            text = f.read()
+    lines = text.splitlines()
+    mats = []
+    for i in range(4):
+        tok = lines[i].split() if i < len(lines) else []
+        if len(tok) != 13 or tok[0] != "P%d:" % i:
+            raise ValueError("calibration line %d is not 'P%d:' followed by 12 numbers: %r"
+                             % (i + 1, i, lines[i] if i < len(lines) else ""))
+        mats.append(np.array([float(v) for v in tok[1:]], np.float64).reshape(3, 4))
+    t = (mats[2][0, 3] - mats[0][0, 3]) / mats[2][0, 0]
+    return Calibration(*mats, t_cam2_cam0_x=float(t))
 
 
 def kitti_result_lines(final, t_cam2_cam0_x):
@@ -779,6 +844,14 @@ def prep_image(img_u8, scale, rgb_input=False, out=None):
     check(L.sb_prep_image(ptr(img_u8.contiguous()), H, W, float(scale), 1 if rgb_input else 0, ptr(out), stream_ptr()),
           "sb_prep_image")
     return out
+
+
+def prep_image_size(H, W, scale):
+    """(Ho, Wo) of the blob prep_image makes of an [H, W] frame at `scale`"""
+    ho, wo = ctypes.c_int(), ctypes.c_int()
+    check(_l.load().sb_prep_image_size(int(H), int(W), float(scale), ctypes.byref(ho), ctypes.byref(wo)),
+          "sb_prep_image_size")
+    return ho.value, wo.value
 
 
 def prep_stereo_pair(left_u8, right_u8, scale, flip, rgb_input=False, out=None):

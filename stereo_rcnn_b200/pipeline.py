@@ -9,7 +9,15 @@ with no host synchronisation, so that it can be captured into a CUDA graph and r
 * `GraphSlot`             : one in-flight unit of work -- its own stream, fixed input buffers, private kernel
                             workspaces (ops.WorkspaceOwner) and the CUDA graph of one step.  Several slots may
                             replay concurrently; they share nothing but the (read-only) weights.
+* `StereoPipeline.step_from_frames` + `EvalInputs` : one image of a test split from its uint8 frames and its
+                            calibration, both in static device buffers, so that one captured graph per frame shape
+                            serves every image of the split.
+* `evaluate`              : test_net.py:118-335 over a split -- the KITTI result files, one per image.
 """
+import glob
+import os
+import time
+
 import numpy as np
 import torch
 
@@ -28,10 +36,12 @@ class StereoPipeline(object):
         self._info = {}
         self.side = torch.cuda.Stream(device=self.dev)
 
-    def im_info(self, B, H, W):
-        key = (B, H, W)
+    def im_info(self, B, H, W, scale=None):
+        """[B, 3] fp32 (H, W, scale) on the device, cached: two frame shapes can give one blob shape at two scales"""
+        scale = self.scale if scale is None else float(np.float32(scale))
+        key = (B, H, W, scale)
         if key not in self._info:
-            self._info[key] = torch.tensor([[H, W, self.scale]] * B, dtype=torch.float32, device=self.dev)
+            self._info[key] = torch.tensor([[H, W, scale]] * B, dtype=torch.float32, device=self.dev)
         return self._info[key]
 
     def step(self, iml, imr, calib4, rois3d, record=None):
@@ -71,15 +81,19 @@ class StereoPipeline(object):
         return record, keep, nkeep, st, dis
 
 
-    def step_with_solver(self, iml, imr, p2, p3, im_hw_orig, cls=1, eval_thresh=0.05, cap=None):
+    def step_with_solver(self, iml, imr, p2, p3, im_hw_orig, cls=1, eval_thresh=0.05, cap=None, scale=None):
         """One pair (B = 1) end to end as test_net.py:120-330 runs it, with the solver stage on the device:
         forward -> decode (+ record) -> per-class NMS -> infer_boundary + border fix-up ->
         solve_x_y_z_theta_from_kpt -> dense_align on the solved poses -> solve_x_y_theta_from_kpt.
         No host synchronisation: detection counts stay on the device (graph-capturable).
+        p2, p3: host 3x4 matrices, or p2 a device calibration [24] (ops.device_calib) and p3 None -- read when the
+        kernels run, so a captured call serves any calibration written there.  scale: im_scale of the blobs (default
+        the pipeline's), rounded to fp32 as im_info holds it.
         -> dict(record [300,33], keep, nkeep, n_solved [1], boxes_all, poses_all, status, best_dis, final [cap,13])"""
         assert iml.shape[0] == 1
         _, _, H, W = iml.shape
-        info = self.im_info(1, H, W)
+        scale = self.scale if scale is None else float(np.float32(scale))
+        info = self.im_info(1, H, W, scale)
         o = self.eng.forward(iml, imr, info)
         R = o["rois_left"].shape[1]
         pbl, pbr, do, pk, rec = ops.test_decode_record(
@@ -90,11 +104,28 @@ class StereoPipeline(object):
         boxes_all, kpts_all, poses_all, src, n = ops.box_solve(
             o["cls_prob"][0], pbl, pbr, do, pk, keep, nkeep, im_hw_orig, p2, p3, cls=cls, eval_thresh=eval_thresh,
             inferred=inferred, cap=cap or R)
-        calib4 = ops.calib_vec(p2, p3)
-        st, dis = ops.dense_align_n(calib4, self.scale, iml[0], imr[0], boxes_all, kpts_all, poses_all, n)
+        calib4 = p2 if torch.is_tensor(p2) else ops.calib_vec(p2, p3)
+        st, dis = ops.dense_align_n(calib4, scale, iml[0], imr[0], boxes_all, kpts_all, poses_all, n)
         final = ops.box_rectify(boxes_all, kpts_all, poses_all, st, dis, n, im_hw_orig, p2, p3)
         return dict(record=rec, keep=keep, nkeep=nkeep, n_solved=n, boxes_all=boxes_all, kpts_all=kpts_all,
                     poses_all=poses_all, src_index=src, status=st, best_dis=dis, final=final)
+
+    def step_from_frames(self, inp, cls=1, eval_thresh=0.05, cap=None):
+        """One test image from the buffers of an EvalInputs: sb_prep_stereo_pair (flip 0) makes the two blobs, then
+        step_with_solver on them with the device calibration and the scale of the frame shape.  Returns what
+        step_with_solver returns.  Outside a stream capture the current stream first waits for inp.load's copies and
+        afterwards marks the buffers as consumed; a captured call holds the kernels only, and whoever replays it calls
+        inp.ready() before and inp.release() after."""
+        capturing = torch.cuda.is_current_stream_capturing()
+        if not capturing:
+            inp.ready()
+        ops.prep_stereo_pair(inp.left_u8, inp.right_u8, inp.scale, inp.flip, rgb_input=inp.rgb_input,
+                             out=(inp.im_left[0], inp.im_right[0]))
+        out = self.step_with_solver(inp.im_left, inp.im_right, inp.calib, None, inp.frame_hw, cls=cls,
+                                    eval_thresh=eval_thresh, cap=cap, scale=inp.scale)
+        if not capturing:
+            inp.release()
+        return out
 
 
 class GraphSlot(object):
@@ -130,3 +161,174 @@ class GraphSlot(object):
         """stage a new pair into the slot's fixed inputs (stream-ordered on the current stream)"""
         self.iml.copy_(iml, non_blocking=non_blocking)
         self.imr.copy_(imr, non_blocking=non_blocking)
+
+
+class EvalInputs(object):
+    """The static buffers of one in-flight step_from_frames at one frame shape: the uint8 frame pair, the device
+    calibration [24] (P2 then P3), a flip flag fixed at 0 and the two blobs.  load() fills the frames and the
+    calibration from pinned host memory on a copy stream of its own.  frame_hw: (H, W) of the camera frames; scale:
+    im_scale of the blobs (target size / shorter side, blob.py:51), unrounded as prep_im_for_blob takes it; rgb_input:
+    the frames are RGB, as image decoders give them, not BGR."""
+
+    def __init__(self, frame_hw, scale, device, rgb_input=True):
+        H, W = int(frame_hw[0]), int(frame_hw[1])
+        self.frame_hw, self.scale, self.rgb_input, self.device = (H, W), float(scale), bool(rgb_input), device
+        host = {"left_u8": torch.empty(H, W, 3, dtype=torch.uint8), "right_u8": torch.empty(H, W, 3, dtype=torch.uint8),
+                "calib": torch.zeros(24, dtype=torch.float64)}
+        self._host = {k: v.pin_memory() for k, v in host.items()}
+        self._dev = {k: torch.zeros_like(v, device=device) for k, v in host.items()}
+        self.left_u8, self.right_u8, self.calib = self._dev["left_u8"], self._dev["right_u8"], self._dev["calib"]
+        self.flip = torch.zeros(1, dtype=torch.int32, device=device)
+        Ho, Wo = ops.prep_image_size(H, W, self.scale)
+        self.im_left = torch.zeros(1, 3, Ho, Wo, dtype=torch.float32, device=device)
+        self.im_right = torch.zeros(1, 3, Ho, Wo, dtype=torch.float32, device=device)
+        self._copy_stream = torch.cuda.Stream(device)
+        self._copied, self._consumed = torch.cuda.Event(), torch.cuda.Event()
+        torch.cuda.current_stream(device).synchronize()        # the zero fills above precede any other stream's use
+
+    def load(self, left, right, calib):
+        """fill the inputs from two uint8 [H,W,3] frames (numpy arrays or tensors) and a calibration (what
+        ops.read_calibration returns, or 24 numbers: P2 then P3): a host copy into pinned memory, then non_blocking
+        copies on the copy stream, which first waits until the step that last read these buffers has finished.  The
+        host waits only for the previous load's copies out of the pinned buffers."""
+        self._copied.synchronize()
+        h = self._host
+        h["left_u8"].copy_(torch.as_tensor(left))
+        h["right_u8"].copy_(torch.as_tensor(right))
+        if hasattr(calib, "p2"):
+            calib = np.concatenate([np.asarray(calib.p2, np.float64).reshape(12), np.asarray(calib.p3, np.float64).reshape(12)])
+        h["calib"].copy_(torch.as_tensor(np.asarray(calib, np.float64).reshape(24)))
+        self._copy_stream.wait_event(self._consumed)
+        with torch.cuda.stream(self._copy_stream):
+            for k, v in h.items():
+                self._dev[k].copy_(v, non_blocking=True)
+            self._copied.record(self._copy_stream)
+
+    def ready(self):
+        """the current stream waits for the copies of the last load()"""
+        torch.cuda.current_stream().wait_event(self._copied)
+
+    def release(self):
+        """the work enqueued so far on the current stream is the last reader of the loaded inputs"""
+        self._consumed.record(torch.cuda.current_stream())
+
+
+def frame_scale(frame_hw, target_size=600):
+    """im_scale of a frame shape (blob.py:51): the unrounded double that prep_im_for_blob takes; im_info and
+    dense_align use it rounded to fp32"""
+    return float(target_size) / float(min(int(frame_hw[0]), int(frame_hw[1])))
+
+
+class _EvalSlot(object):
+    """one (frame shape, slot) of evaluate: inputs, workspaces, stream, graph, pinned results and their event"""
+
+    def __init__(self, pipe, frame_hw, target_size, rgb_input):
+        self.inp = EvalInputs(frame_hw, frame_scale(frame_hw, target_size), pipe.dev, rgb_input=rgb_input)
+        self.ws = ops.WorkspaceOwner()
+        self.stream = torch.cuda.Stream(device=pipe.dev)
+        self.runner = None
+        self.final_h = self.n_h = None
+        self.done = torch.cuda.Event()
+
+    def step(self, pipe):
+        """step_from_frames, then its final rows and n_solved copied to this slot's pinned host buffers"""
+        out = pipe.step_from_frames(self.inp)
+        if self.final_h is None:
+            self.final_h = torch.zeros(out["final"].shape, dtype=out["final"].dtype).pin_memory()
+            self.n_h = torch.zeros(1, dtype=torch.int32).pin_memory()
+        self.final_h.copy_(out["final"], non_blocking=True)
+        self.n_h.copy_(out["n_solved"], non_blocking=True)
+        return out
+
+
+def evaluate(pipe, entries, frames, calib, result_dir, inflight=1, use_graph=True, target_size=600, rgb_input=True,
+             name=None, log=print, empty_files=False):
+    """The test loop of test_net.py:118-335 over a split: per entry the frames and the calibration, forward, decode,
+    per-class NMS, infer_boundary, solve_x_y_z_theta_from_kpt, align_parallel, solve_x_y_theta_from_kpt (all in
+    StereoPipeline.step_from_frames), then write_detection_results' lines (kitti_utils.py:440-460) in
+    result_dir/data/<name>.txt -- the files a KITTI evaluation tool reads.
+
+    frames(entry) -> (left, right) uint8 [H,W,3] arrays (RGB unless rgb_input is False); calib(entry) -> what
+    ops.read_calibration returns; name(entry) -> the file stem (default entry["image_id"]).  The scale of a frame shape
+    is target_size / its shorter side (blob.py:51).
+
+    Each (frame shape, slot) has its own EvalInputs, workspaces, stream and -- with use_graph -- one CUDA graph,
+    captured after a first eager step; the graph also copies `final` and `n_solved` to the slot's pinned host
+    buffers.  Entries go round-robin over `inflight` slots; the next entry's frames are read and copied while the
+    current step runs, and a slot's results are read after its event, `inflight` entries late, so the steady state
+    has no device-wide synchronise.  With use_graph the pipeline must be built with throughput=True (one chain per
+    step, no stream forks inside it; the slots supply the concurrency), which is checked before any work.
+
+    Files are written in entry order.  As in the reference, an image without a detection gets no file; with
+    empty_files every evaluated image gets one (evaluation tools read one file per image of the split).  Where the
+    reference deletes its result directory, this refuses to start when result_dir/data already holds .txt files.
+    -> dict(images, lines, files, graphs, write_s: host seconds spent formatting and writing the files)"""
+    data_dir = os.path.join(result_dir, "data")
+    if glob.glob(os.path.join(data_dir, "*.txt")):
+        raise FileExistsError("%s already holds result files; evaluate writes into an empty directory" % data_dir)
+    if inflight < 1:
+        raise ValueError("inflight must be >= 1")
+    if use_graph and pipe.eng.forks:
+        raise ValueError("evaluate captures its graphs from a pipeline built with throughput=True")
+    os.makedirs(data_dir, exist_ok=True)
+    name = name or (lambda e: e["image_id"])
+    states = {}
+    pending = [None] * inflight                  # per slot: (entry index, _EvalSlot, t_cam2_cam0_x, file stem)
+    summary = dict(images=0, lines=0, files=0, graphs=0, write_s=0.0)
+
+    def load(k):
+        left, right = frames(entries[k])
+        hw = (int(left.shape[0]), int(left.shape[1]))
+        key = (hw, k % inflight)
+        if key not in states:
+            states[key] = _EvalSlot(pipe, hw, target_size, rgb_input)
+        st = states[key]
+        c = calib(entries[k])
+        st.inp.load(left, right, c)
+        return st, c.t_cam2_cam0_x
+
+    def launch(st):
+        with torch.cuda.stream(st.stream), torch.no_grad(), ops.workspace_owner(st.ws):
+            if not use_graph or st.runner is None:
+                st.step(pipe)                    # eager; the first step on a slot also creates its workspaces
+                if use_graph:
+                    from .engine import GraphRunner
+                    st.runner = GraphRunner(lambda: st.step(pipe), [], warmup=0)
+                    summary["graphs"] += 1
+            else:
+                st.inp.ready()
+                st.runner()
+                st.inp.release()
+            st.done.record(st.stream)
+
+    def finish(p):
+        k, st, t_x, stem = p
+        st.done.synchronize()
+        t0 = time.perf_counter()
+        n = int(st.n_h[0])
+        lines = ops.kitti_result_lines(st.final_h[:n], t_x)
+        if lines or empty_files:
+            with open(os.path.join(data_dir, stem + ".txt"), "w") as f:
+                f.write("".join(lines))
+            summary["files"] += 1
+        summary["write_s"] += time.perf_counter() - t0
+        summary["images"] += 1
+        summary["lines"] += len(lines)
+
+    n = len(entries)
+    nxt = load(0) if n else None
+    for k in range(n):
+        st, t_x = nxt
+        if pending[k % inflight] is not None:    # entry k - inflight: read before this slot's buffers are reused
+            finish(pending[k % inflight])
+        launch(st)
+        pending[k % inflight] = (k, st, t_x, str(name(entries[k])))
+        if k + 1 < n:
+            nxt = load(k + 1)                    # host reads + H2D of the next entry overlap this step
+    for j in range(inflight):                    # the last ones, in entry order
+        p = pending[(n + j) % inflight]
+        if p is not None:
+            finish(p)
+    log("evaluate: %d images, %d lines in %d files, %d graphs" % (summary["images"], summary["lines"],
+                                                                 summary["files"], summary["graphs"]))
+    return summary
