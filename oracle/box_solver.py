@@ -164,10 +164,17 @@ class Problem(object):
         return np.array([x, y, z, th]) if self.z_fixed is None else np.array([x, y, th])
 
 
+def rejected(box_left, kpts):
+    """the rejection rules of box_estimator.py:187 as test_net.py:287-295 evaluates them: the box is a float32 numpy
+    row and the keypoints a float32 torch row, so each difference is rounded to float32 before it is compared"""
+    b, k = np.asarray(box_left, np.float32), np.asarray(kpts, np.float32)
+    return bool(k[4] - k[3] < 3 or b[2] - b[0] < 10 or b[3] - b[1] < 10)
+
+
 def solve_x_y_z_theta_from_kpt(im_shape, p2, p3, alpha, dim, box_left, box_right, kpts):
     """box_estimator.py:169-385 -> (status, state[4] or 0)"""
     from scipy.optimize import minimize
-    if kpts[4] - kpts[3] < 3 or box_left[2] - box_left[0] < 10 or box_left[3] - box_left[1] < 10:
+    if rejected(box_left, kpts):
         return 0, 0
     pb = Problem(im_shape, p2, p3, alpha, dim, box_left, box_right, kpts)
     res = minimize(pb.objective, pb.init(), method="Newton-CG", jac=pb.gradient, options={"disp": False})

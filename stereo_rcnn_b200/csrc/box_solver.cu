@@ -89,8 +89,7 @@ box_solve_kernel(SolveArgs a, int cap, float* __restrict__ boxes_all /*[cap,5]*/
             if (__fsub_rn(kp[4], kp[3]) < __fmul_rn(0.5f, __fsub_rn(i1, i0))) { kp[3] = i0; kp[4] = i1; }
         }
         box[0] = bl[0]; box[1] = bl[1]; box[2] = bl[2]; box[3] = bl[3]; box[4] = score;
-        if (score > a.eval_thresh &&
-            !((double)kp[4] - (double)kp[3] < 3 || (double)box[2] - (double)box[0] < 10 || (double)box[3] - (double)box[1] < 10)) {
+        if (score > a.eval_thresh && !sb_box_rejected(box, kp)) {
             const double alpha = atan2((double)dm[3], (double)dm[4]);
             const double dim[3] = {dm[0], dm[1], dm[2]};
             const double bld[4] = {box[0], box[1], box[2], box[3]}, brd[4] = {br[0], br[1], br[2], br[3]};

@@ -33,6 +33,18 @@ struct SbBoxProblem {
     double z_fixed, disparity;
 };
 
+// box_estimator.py:187's rejection rules on the float32 box [x1,y1,x2,y2] and keypoints [.., left border, right
+// border]: 1 = not solved.  test_net.py passes the box as a float32 numpy row and the keypoints as a float32 torch row,
+// so each difference is rounded to float32 before it is compared: a difference just below the threshold can round up
+// to it, and then the reference solves the detection.  __fsub_rn keeps the device from contracting or widening it.
+SB_HD int sb_box_rejected(const float* box, const float* kp) {
+#if defined(__CUDA_ARCH__)
+    return __fsub_rn(kp[4], kp[3]) < 3.f || __fsub_rn(box[2], box[0]) < 10.f || __fsub_rn(box[3], box[1]) < 10.f;
+#else
+    return kp[4] - kp[3] < 3.f || box[2] - box[0] < 10.f || box[3] - box[1] < 10.f;
+#endif
+}
+
 SB_HD int sb_bb2viewpoint(double alpha) {       // box_estimator.py:15-42
     const double kPi = 3.141592653589793;
     alpha = alpha * 180.0 / kPi;

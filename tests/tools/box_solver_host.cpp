@@ -21,6 +21,9 @@ int box_solve_host(int im_h, int im_w, const double* p2, const double* p3, doubl
     return 0;
 }
 
+// the status rules of box_estimator.py:187 on float32 inputs: 1 = rejected (box [4], kpts [5])
+int box_rejected_host(const float* box, const float* kpts) { return sb_box_rejected(box, kpts); }
+
 // objective (kpt_scale 2 = the reference's f) and the reference-style gradient (sum 2 r_i dr_i with the keypoint
 // derivative halved) at a given state, for golden comparison
 int box_eval_host(int im_h, int im_w, const double* p2, const double* p3, double alpha, const double* dim,
