@@ -613,6 +613,43 @@ int sb_random_words(unsigned long long seed, const unsigned long long* step, uns
                     size_t n, sb_stream_t stream);
 int sb_step_advance(unsigned long long* step, sb_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * KITTI average precision of a split (Car), the KITTI object devkit's evaluate_object restated (DESIGN.md §9).
+ *
+ * Rows: SB_KITTI_ROW doubles per label / result line -- trunc, occ, alpha, x1, y1, x2, y2, h, w, l, x, y, z, cos(ry),
+ * sin(ry), score (0 for labels) -- and an int32 code per row: 0 Car, 1 Van, 2 DontCare, 3 anything else.  Images are
+ * in CSR form: the gt rows of image i are gt_off[i] .. gt_off[i+1], its detection rows det_off[i] .. det_off[i+1], and
+ * its pairs pair_off[i] .. pair_off[i+1], with pair_off[i+1] - pair_off[i] = n_det(i) * n_gt(i) (int64 offsets in
+ * DEVICE memory, offsets[0] = 0).  Rows must be finite.
+ * sb_kitti_overlaps -- the devkit's boxoverlap, groundBoxOverlap and box3DOverlap for every (detection, gt) pair of
+ *   every image: the pair (j, i) of image k is element pair_off[k] + j * n_gt(k) + i of each output.  A DontCare gt
+ *   column holds intersection / area(det) (the devkit's criterion 0), every other column intersection / union.
+ * sb_kitti_eval -- eval_class for 3 metrics (2D, BEV, 3D) x n_bars IoU bars x 3 difficulties (easy, moderate, hard):
+ *   configuration c = (metric * n_bars + bar) * 3 + difficulty, C = 9 * n_bars.  computeStatistics without and with
+ *   false positives, getThresholds, and the precision / recall / orientation-similarity curves.  Outputs per
+ *   configuration: thresholds [C,41] (0 past n_thresholds[c]), n_thresholds [C] int32, tp / fp / fn [C,41] int64,
+ *   sim [C,41] (summed orientation similarity), precision / recall / aos [C,41] (precision and aos replaced by their
+ *   maxima to the right), ap [C,4] = (precision R11, precision R40, aos R11, aos R40) in percent, n_gt [C] int64.
+ *   bars: host array of n_bars (1..SB_KITTI_MAX_BARS) values in [0, 1].  The workspace is 256-byte aligned and at
+ *   least sb_kitti_eval_workspace_bytes (0 for sizes it refuses).
+ * SB_EINVAL before any launch for a null pointer, n_images < 1, a negative row or pair count, a bar outside [0, 1] or
+ *   a workspace that is too small or misaligned.                                                                  */
+#define SB_KITTI_ROW 16
+#define SB_KITTI_MAX_THRESHOLDS 41
+#define SB_KITTI_MAX_BARS 4
+
+int sb_kitti_overlaps(const double* gt, const int* gt_code, const double* det, const long long* gt_off,
+                      const long long* det_off, const long long* pair_off, int n_images, long long n_pairs,
+                      double* ov_2d, double* ov_bev, double* ov_3d, sb_stream_t stream);
+size_t sb_kitti_eval_workspace_bytes(int n_images, long long n_gt_rows, long long n_det_rows, long long n_pairs,
+                                     int n_bars);
+int sb_kitti_eval(const double* gt, const int* gt_code, const double* det, const int* det_code,
+                  const long long* gt_off, const long long* det_off, const long long* pair_off, int n_images,
+                  long long n_gt_rows, long long n_det_rows, long long n_pairs, const double* bars, int n_bars,
+                  void* workspace, size_t workspace_bytes, double* thresholds, int* n_thresholds, long long* tp,
+                  long long* fp, long long* fn, double* sim, double* precision, double* recall, double* aos,
+                  double* ap, long long* n_gt, sb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -179,6 +179,11 @@ _SIGS = {
     "sb_train_gt": (c_int, [c_void_p] * 8 + [c_int, c_int, c_float, c_int] + [c_void_p] * 6 + [c_void_p]),
     "sb_random_words": (c_int, [ctypes.c_ulonglong, c_void_p, ctypes.c_uint, c_void_p, c_size_t, c_void_p]),
     "sb_step_advance": (c_int, [c_void_p, c_void_p]),
+    # KITTI average precision of a split
+    "sb_kitti_overlaps": (c_int, [c_void_p] * 6 + [c_int, c_ll] + [c_void_p] * 3 + [c_void_p]),
+    "sb_kitti_eval_workspace_bytes": (c_size_t, [c_int, c_ll, c_ll, c_ll, c_int]),
+    "sb_kitti_eval": (c_int, [c_void_p] * 7 + [c_int, c_ll, c_ll, c_ll, ctypes.POINTER(c_double), c_int, c_void_p,
+                              c_size_t] + [c_void_p] * 11 + [c_void_p]),
 }
 
 EXPORTS = tuple(_SIGS)

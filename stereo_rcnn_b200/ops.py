@@ -894,3 +894,61 @@ def round_tf32_(w):
 def unbias(x):
     """exact fp32 view of a tensor stored pre-biased (out_mode 2); debugging / tests only"""
     return (x.view(torch.int32) - 0x1000).view(torch.float32)
+
+
+# ------------------------------------------------------------- KITTI evaluation ----
+KITTI_ROW, KITTI_T = 16, 41                       # SB_KITTI_ROW, SB_KITTI_MAX_THRESHOLDS
+
+
+def kitti_overlaps(gt, gt_code, det, gt_off, det_off, pair_off, n_pairs):
+    """sb_kitti_overlaps: rows fp64 [n,16], codes int32, CSR offsets int64 [n_images+1] (device), n_pairs =
+    pair_off[-1] -> (ov_2d, ov_bev, ov_3d) fp64 [n_pairs], image k's pair (det j, gt i) at pair_off[k] + j * n_gt(k) + i"""
+    L = _l.load()
+    n_pairs = int(n_pairs)
+    dev = gt_off.device
+    out = torch.empty(3, max(n_pairs, 1), dtype=torch.float64, device=dev)
+    check(L.sb_kitti_overlaps(ptr(gt), ptr(gt_code), ptr(det), ptr(gt_off), ptr(det_off), ptr(pair_off),
+                              gt_off.numel() - 1, n_pairs, ptr(out[0]), ptr(out[1]), ptr(out[2]), stream_ptr()),
+          "sb_kitti_overlaps")
+    return out[0, :n_pairs], out[1, :n_pairs], out[2, :n_pairs]
+
+
+KITTI_OUTPUTS = (("thresholds", torch.float64, KITTI_T), ("n_thresholds", torch.int32, 0), ("tp", torch.int64, KITTI_T),
+                 ("fp", torch.int64, KITTI_T), ("fn", torch.int64, KITTI_T), ("sim", torch.float64, KITTI_T),
+                 ("precision", torch.float64, KITTI_T), ("recall", torch.float64, KITTI_T),
+                 ("aos", torch.float64, KITTI_T), ("ap", torch.float64, 4), ("n_gt", torch.int64, 0))
+
+
+def kitti_eval(gt, gt_code, det, det_code, gt_off, det_off, pair_off, n_pairs, bars, out=None):
+    """sb_kitti_eval over a packed split (see kitti_overlaps; n_pairs = pair_off[-1], known on the host) ->
+    dict of the outputs, configuration c = (metric * len(bars) + bar) * 3 + difficulty.  out: a dict of the same
+    tensors to write into (kitti_eval_outputs)"""
+    L = _l.load()
+    n_images = gt_off.numel() - 1
+    ng, nd = gt_code.numel(), det_code.numel()
+    dev = gt_off.device
+    nb = L.sb_kitti_eval_workspace_bytes(n_images, ng, nd, int(n_pairs), len(bars))
+    if nb == 0:
+        raise ValueError("sb_kitti_eval refuses these sizes (%d images, %d bars)" % (n_images, len(bars)))
+    ws = workspace(nb + 256, dev, "kitti_eval")
+    base = (-ws.data_ptr()) % 256
+    out = out or kitti_eval_outputs(len(bars), dev)
+    b = (ctypes.c_double * len(bars))(*[float(v) for v in bars])
+    check(L.sb_kitti_eval(ptr(gt), ptr(gt_code), ptr(det), ptr(det_code), ptr(gt_off), ptr(det_off), ptr(pair_off),
+                          n_images, ng, nd, int(n_pairs), b, len(bars), ctypes.c_void_p(ws.data_ptr() + base), nb,
+                          *[ptr(out[k]) for k, _t, _n in KITTI_OUTPUTS], stream_ptr()), "sb_kitti_eval")
+    return out
+
+
+def kitti_eval_outputs(n_bars, device):
+    """the output tensors of kitti_eval for n_bars bars: views into one device buffer (one D2H copies them all)"""
+    C = 9 * n_bars
+    sizes = [C * max(n, 1) for _k, _t, n in KITTI_OUTPUTS]
+    buf = torch.zeros(sum(sizes), dtype=torch.float64, device=device)
+    out, o = {}, 0
+    for (k, t, n), s in zip(KITTI_OUTPUTS, sizes):
+        v = buf[o:o + s].view(t)
+        out[k] = v.view(C, n) if n else v[:C]
+        o += s
+    out["_buffer"] = buf
+    return out

@@ -12,7 +12,8 @@ with no host synchronisation, so that it can be captured into a CUDA graph and r
 * `StereoPipeline.step_from_frames` + `EvalInputs` : one image of a test split from its uint8 frames and its
                             calibration, both in static device buffers, so that one captured graph per frame shape
                             serves every image of the split.
-* `evaluate`              : test_net.py:118-335 over a split -- the KITTI result files, one per image.
+* `evaluate`              : test_net.py:118-335 over a split -- the KITTI result files, one per image, and with
+                            `labels` their Car AP (kitti_eval).
 """
 import glob
 import os
@@ -242,7 +243,7 @@ class _EvalSlot(object):
 
 
 def evaluate(pipe, entries, frames, calib, result_dir, inflight=1, use_graph=True, target_size=600, rgb_input=True,
-             name=None, log=print, empty_files=False):
+             name=None, log=print, empty_files=False, labels=None):
     """The test loop of test_net.py:118-335 over a split: per entry the frames and the calibration, forward, decode,
     per-class NMS, infer_boundary, solve_x_y_z_theta_from_kpt, align_parallel, solve_x_y_theta_from_kpt (all in
     StereoPipeline.step_from_frames), then write_detection_results' lines (kitti_utils.py:440-460) in
@@ -262,7 +263,11 @@ def evaluate(pipe, entries, frames, calib, result_dir, inflight=1, use_graph=Tru
     Files are written in entry order.  As in the reference, an image without a detection gets no file; with
     empty_files every evaluated image gets one (evaluation tools read one file per image of the split).  Where the
     reference deletes its result directory, this refuses to start when result_dir/data already holds .txt files.
-    -> dict(images, lines, files, graphs, write_s: host seconds spent formatting and writing the files)"""
+
+    labels(entry) -> the image's KITTI label file (a path or its text): when given, the lines written for each image
+    are scored against it (kitti_eval.KittiEval, on the device, after the loop), images without a detection included,
+    and summary["ap"] holds KittiEval.result() -- the Car AP of exactly the files written.
+    -> dict(images, lines, files, graphs, write_s: host seconds spent formatting and writing the files[, ap])"""
     data_dir = os.path.join(result_dir, "data")
     if glob.glob(os.path.join(data_dir, "*.txt")):
         raise FileExistsError("%s already holds result files; evaluate writes into an empty directory" % data_dir)
@@ -275,6 +280,10 @@ def evaluate(pipe, entries, frames, calib, result_dir, inflight=1, use_graph=Tru
     states = {}
     pending = [None] * inflight                  # per slot: (entry index, _EvalSlot, t_cam2_cam0_x, file stem)
     summary = dict(images=0, lines=0, files=0, graphs=0, write_s=0.0)
+    scorer = None
+    if labels is not None:
+        from .kitti_eval import KittiEval
+        scorer = KittiEval(pipe.dev)
 
     def load(k):
         left, right = frames(entries[k])
@@ -312,6 +321,8 @@ def evaluate(pipe, entries, frames, calib, result_dir, inflight=1, use_graph=Tru
                 f.write("".join(lines))
             summary["files"] += 1
         summary["write_s"] += time.perf_counter() - t0
+        if scorer is not None:
+            scorer.add(labels(entries[k]), "".join(lines))
         summary["images"] += 1
         summary["lines"] += len(lines)
 
@@ -331,4 +342,8 @@ def evaluate(pipe, entries, frames, calib, result_dir, inflight=1, use_graph=Tru
             finish(p)
     log("evaluate: %d images, %d lines in %d files, %d graphs" % (summary["images"], summary["lines"],
                                                                  summary["files"], summary["graphs"]))
+    if scorer is not None and n:
+        summary["ap"] = scorer.result()
+        log("evaluate: Car AP|R11 (easy, moderate, hard) 2D %s, AOS %s, BEV %s, 3D %s at IoU 0.7" % tuple(
+            "/".join("%.2f" % v for v in summary["ap"][m][0.7][:, 0]) for m in ("bbox", "aos", "bev", "3d")))
     return summary

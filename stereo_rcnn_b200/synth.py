@@ -255,3 +255,56 @@ def synth_train_rois(gt_left, R, H, W, seed, near_gt=0.34, jitter=6.0, disparity
     right[:, :, 1] -= disparity
     right[:, :, 3] -= disparity
     return out, right
+
+
+def kitti_split(n_images, seed=0, n_cars=4, n_dets=30):
+    """A seeded synthetic KITTI split as text: per image about n_cars Cars, a Van, a Pedestrian and two DontCare
+    label lines, and about n_dets result lines -- jittered copies of the labelled objects (orientations across +-pi
+    included) and detections away from them -> [(label_text, result_text)]"""
+    rs = np.random.RandomState(seed)
+
+    def obj(kind):
+        z = rs.uniform(5.0, 60.0)
+        x = rs.uniform(-15.0, 15.0)
+        h, w, l = {"Car": (1.5, 1.6, 3.9), "Van": (2.2, 1.9, 5.0), "Pedestrian": (1.7, 0.6, 0.8)}[kind]
+        h, w, l = h * rs.uniform(0.9, 1.1), w * rs.uniform(0.9, 1.1), l * rs.uniform(0.9, 1.1)
+        u = 621.0 + 720.0 * x / z
+        bh = 720.0 * h / z
+        bw = 720.0 * max(w, l) / z
+        y = 1.65 + rs.uniform(-0.2, 0.2)
+        v2 = 175.0 + 720.0 * y / z
+        return [float(rs.choice([0.0, 0.1, 0.15, 0.3, 0.6])), int(rs.choice([0, 1, 2, 3])), rs.uniform(-np.pi, np.pi),
+                u - bw / 2, v2 - bh, u + bw / 2, v2, h, w, l, x, y, z, rs.uniform(-np.pi, np.pi)]
+
+    def line(kind, r, score=None):
+        s = "%s %.2f %d %.2f %.2f %.2f %.2f %.2f %.2f %.2f %.2f %.2f %.2f %.2f %.2f" % tuple([kind] + list(r))
+        return s + (" %.4f\n" % score if score is not None else "\n")
+
+    split = []
+    for _ in range(n_images):
+        kinds = ["Car"] * max(0, n_cars + rs.randint(-1, 2)) + ["Van", "Pedestrian"]
+        gts = [(k, obj(k)) for k in kinds]
+        labels = [line(k, r) for k, r in gts]
+        for _d in range(2):
+            x1, y1 = rs.uniform(0, 1100), rs.uniform(100, 300)
+            labels.append("DontCare -1 -1 -10 %.2f %.2f %.2f %.2f -1 -1 -1 -1000 -1000 -1000 -10\n"
+                          % (x1, y1, x1 + rs.uniform(10, 120), y1 + rs.uniform(10, 60)))
+        dets = []
+        while len(dets) < n_dets + rs.randint(-3, 4):
+            if rs.rand() < 0.6:
+                k, r = gts[rs.randint(len(gts))]
+                r = list(r)
+                j = rs.uniform(0.0, 0.15)
+                bw, bh = r[5] - r[3], r[6] - r[4]
+                r[3:7] = [r[3] + rs.randn() * j * bw, r[4] + rs.randn() * j * bh, r[5] + rs.randn() * j * bw,
+                          r[6] + rs.randn() * j * bh]
+                r[10] += rs.randn() * j * r[9]
+                r[12] += rs.randn() * j * r[9]
+                r[13] = (r[13] + rs.randn() * 0.3 + np.pi) % (2 * np.pi) - np.pi
+                r[2] = (r[2] + rs.randn() * 0.3 + np.pi) % (2 * np.pi) - np.pi
+                k = "Car" if rs.rand() < 0.9 else k
+            else:
+                k, r = "Car", obj("Car")
+            dets.append(line(k, r, rs.uniform(0.05, 1.0)))
+        split.append(("".join(labels), "".join(dets)))
+    return split
