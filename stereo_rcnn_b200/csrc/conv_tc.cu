@@ -29,15 +29,18 @@
 //     arbitrary n/h/w strides and channel offset (RPN L|R concat, deconv scatter).  All loads of a column step (both
 //     rows: residual, the four upsample taps, scale / shift) are issued before its first store.
 //   * residual epilogue by TMA (fp16 operands, forward: conv3 of every bottleneck, HBM-bound): per consumer warpgroup
-//     a shared-memory buffer of its 64 rows -- BLOCK_N / 32 fp32 boxes of 64 x 32 (residual in, result out in place)
-//     and ceil(BLOCK_N / 64) fp16 boxes of 64 x 64 (the twin), 128-byte swizzled -- on its own full / empty mbarrier
-//     pair.  The producer requests tile t's residual boxes right after the first min(K-steps, stages) operand loads of
-//     tile t, so they land during tile t's main loop.  The consumers add the accumulators in place, write the twin,
-//     fence the async proxy and sync the warpgroup (named barrier); one thread issues the bulk tensor stores, waits
-//     until they have read the buffer (cp.async.bulk.wait_group.read) and releases it, and the warpgroup goes on to
-//     the next tile's MMAs while the stores drain to HBM.  Shared memory of a 128-wide residual tile: 4 operand
-//     stages of 32 KB + 2 warpgroups x (32 KB fp32 + 16 KB fp16) = 96 KB of epilogue buffers (64-wide: 7 x 24 KB +
-//     48 KB; 32-wide: 9 x 20 KB + 32 KB).  The TF32 mode and the data-gradient variants keep the register epilogue.
+//     a ring of slots with its own full / empty mbarriers, each slot one 32-column chunk of the warpgroup's 64 rows --
+//     an fp32 box of 64 x 32 (residual in, result out in place, 128-byte swizzle) and an fp16 box of 64 x 32 (the
+//     twin, 64-byte swizzle).  Warps 9 and 10 are the residual producers of the two warpgroups: each loads its
+//     warpgroup's chunks in (tile, chunk) order as soon as a slot is empty, so the next tile's residual streams in
+//     under this tile's last chunks and the next main loop; the operand producer never waits on the ring.  Per chunk
+//     the consumers add the accumulators in place, write the twin, fence the async proxy and sync the warpgroup
+//     (named barrier); one thread issues the chunk's bulk tensor stores as one group and returns the previous chunk's
+//     slot once its group has read it (cp.async.bulk.wait_group.read 1; the last chunk of a tile is returned under
+//     the next tile's first MMAs).  Both sides step through every chunk of every tile, stored or not (rows past M,
+//     columns past Cout, a warpgroup without rows in the last tile).  Shared memory of a 128-wide residual tile: 4
+//     operand stages of 32 KB + 2 warpgroups x 4 slots x 12 KB = 96 KB of rings (64-wide: 6 x 24 KB + 2 x 3 x 12 KB;
+//     32-wide: 7 x 20 KB + 2 x 3 x 12 KB).  The TF32 mode and the data-gradient variants keep the register epilogue.
 //   * programmatic dependent launch: the prologue (barrier init, descriptor prefetch) overlaps the previous
 //     kernel's tail; dependents are released after the CTA's last operand loads are issued.
 //   * optional per-CTA phase trace (sb_conv_trace) for tools/conv_trace.py.
@@ -85,21 +88,26 @@ __device__ __forceinline__ unsigned long long gtimer() {
 }
 constexpr int kTraceWords = 16, kTraceCtas = 304;
 
-// TMA residual epilogue (fp16-operand forward with a residual): per consumer warpgroup, its 64 rows of the tile as
-// BLOCK_N / 32 fp32 boxes [64 rows][32 columns] (residual in, fp32 result out, in place) and ceil(BLOCK_N / 64) fp16
-// boxes [64 rows][64 columns] (the twin); every box is 64 x 128 bytes, 128-byte swizzled.
-constexpr uint32_t kEpiBox = 64 * 128;
+// TMA residual epilogue (fp16-operand forward with a residual): per consumer warpgroup, a ring of epi_slots(BLOCK_N)
+// slots, each one 32-column chunk of the warpgroup's 64 tile rows: an fp32 box [64 rows][32 columns] (residual in,
+// fp32 result out, in place; 128-byte rows, 128-byte swizzle) and an fp16 box [64 rows][32 columns] (the twin; 64-byte
+// rows, 64-byte swizzle).  Warps 9 and 10 are the residual producers of warpgroups 0 and 1.
+constexpr uint32_t kEpiBox = 64 * 128, kTwinBox = 64 * 64, kSlotBytes = kEpiBox + kTwinBox;
+constexpr int kResProducerWarps = 2;
+constexpr int kResThreads = kThreads + 32 * kResProducerWarps;
 constexpr bool tma_epilogue(bool has_res, bool in16, bool mask) { return has_res && in16 && !mask; }
-constexpr uint32_t epi_res_bytes(int block_n) { return (uint32_t)(block_n / 32) * kEpiBox; }
-constexpr uint32_t epi_twin_bytes(int block_n) { return (uint32_t)((block_n + 63) / 64) * kEpiBox; }
-constexpr uint32_t epi_bytes(int block_n) { return 2 * (epi_res_bytes(block_n) + epi_twin_bytes(block_n)); }
+constexpr int epi_slots(int block_n) { return block_n == 128 ? 4 : 3; }
+constexpr int conv_threads(bool stem, bool tma_epi) { return stem ? kStemThreads : tma_epi ? kResThreads : kThreads; }
 
-constexpr size_t conv_smem(int block_n, int stages, uint32_t epi) {
-    return (size_t)stages * (BLOCK_M * kRowBytes + block_n * kRowBytes) + epi + 1024 + (2 * stages + 4) * 8;
+// operand stages, then (slots > 0) both warpgroups' epilogue rings, the 1024-byte alignment pad and the mbarriers
+// (operand ring, epilogue rings, the residual producers' start)
+constexpr size_t conv_smem(int block_n, int stages, int slots) {
+    return (size_t)stages * (BLOCK_M * kRowBytes + block_n * kRowBytes) + (size_t)2 * slots * kSlotBytes + 1024 +
+           (2 * stages + 4 * slots + 1) * 8;
 }
 
 template <int BLOCK_N, int kStages, bool HAS_RES, bool HAS_UP, bool IN16, bool STEM = false, bool MASK = false>
-__global__ void __launch_bounds__(STEM ? kStemThreads : kThreads, 1)
+__global__ void __launch_bounds__(conv_threads(STEM, tma_epilogue(HAS_RES, IN16, MASK)), 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                const __grid_constant__ CUtensorMap map_r, const __grid_constant__ CUtensorMap map_o,
                const __grid_constant__ CUtensorMap map_o16, const TcParams p) {
@@ -110,14 +118,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     constexpr uint32_t kABytes = BLOCK_M * kRowBytes, kBBytes = BLOCK_N * kRowBytes;
     constexpr int BLOCK_K = IN16 ? 64 : 32;     // elements per K-step
     constexpr uint32_t kStageBytes = kABytes + kBBytes;
-    constexpr uint32_t kResWg = epi_res_bytes(BLOCK_N), kTwinWg = epi_twin_bytes(BLOCK_N);
+    constexpr int kSlots = kTmaEpi ? epi_slots(BLOCK_N) : 0;     // epilogue ring slots per consumer warpgroup
+    constexpr int kChunks = BLOCK_N / 32;                        // ring entries per tile and warpgroup
+    // a chunk's slot is released while the next chunk is processed, so the producer needs a second slot to load it
+    static_assert(!kTmaEpi || kSlots >= 2, "epilogue ring of at least two slots");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t* epi = smem + kStages * kStageBytes;                  // [2][kResWg] fp32 boxes, then [2][kTwinWg] fp16
-    uint64_t* full = reinterpret_cast<uint64_t*>(epi + (kTmaEpi ? epi_bytes(BLOCK_N) : 0));
+    uint8_t* epi = smem + kStages * kStageBytes;                  // [2 warpgroups][kSlots][kSlotBytes]
+    uint64_t* full = reinterpret_cast<uint64_t*>(epi + 2 * kSlots * kSlotBytes);
     uint64_t* empty = full + kStages;
-    uint64_t* res_full = empty + kStages;     // [2]: the warpgroup's residual boxes have landed
-    uint64_t* res_empty = res_full + 2;       // [2]: its output stores have read the buffer
+    uint64_t* slot_full = empty + kStages;         // [2][kSlots]: the chunk's residual box has landed
+    uint64_t* slot_empty = slot_full + 2 * kSlots; // [2][kSlots]: the chunk's output stores have read the slot
+    uint64_t* res_go = slot_empty + 2 * kSlots;    // the first tile's first operand loads are issued
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const sb_conv_desc& d = p.d;
@@ -137,12 +149,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             mbar_init(&full[i], STEM ? 1 + 32 * kStemGatherWarps : 1);
             mbar_init(&empty[i], kConsumerWarps);
         }
-        if (kTmaEpi) {
-            for (int g = 0; g < 2; ++g) {
-                mbar_init(&res_full[g], 1);      // the producer's expect_tx arrival
-                mbar_init(&res_empty[g], 1);     // the warpgroup's store thread
-            }
+        for (int i = 0; i < 2 * kSlots; ++i) {
+            mbar_init(&slot_full[i], 1);         // the residual producer's expect_tx arrival
+            mbar_init(&slot_empty[i], 1);        // the warpgroup's store thread
         }
+        if (kTmaEpi) mbar_init(res_go, 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -157,11 +168,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         // ===================== TMA producer =====================
         if (lane == 0) {
             int stage = 0;
-            uint32_t phase = 0, rphase = 0;
-            // the tile's residual boxes follow its first min(K-steps, stages) operand loads: those need only free
-            // stages, so they are in flight while the consumers finish the previous tile's epilogue, and the
-            // residual (which waits for that epilogue's stores to leave the buffer) lands during this main loop
-            const int kb_res = (p.num_k_blocks < kStages ? p.num_k_blocks : kStages) - 1;
+            uint32_t phase = 0;
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
                 const int mt = tile / p.num_n_tiles, nt = tile - mt * p.num_n_tiles;
                 int n_img = 0, h0 = 0, w0 = 0;
@@ -199,23 +206,39 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                     }
                     tma_load_2d(&map_b, &full[stage], sa + kABytes, tap * d.Cin + c0, nt * BLOCK_N);
                     if (++stage == kStages) { stage = 0; phase ^= 1; }
-                    if (kTmaEpi && kb == kb_res) {
-                        // rows past M and columns past Cout are zero-filled (and still counted in the bytes)
-                        for (int g = 0; g < 2; ++g) {
-                            mbar_wait(&res_empty[g], rphase ^ 1);
-                            mbar_expect_tx(&res_full[g], kResWg);
-                            for (int b = 0; b < BLOCK_N / 32; ++b)
-                                tma_load_2d(&map_r, &res_full[g], epi + g * kResWg + b * kEpiBox, nt * BLOCK_N + 32 * b,
-                                            mt * BLOCK_M + 64 * g);
-                        }
-                        rphase ^= 1;
-                    }
+                    // the residual producers start once the first tile's first min(K-steps, stages) operand loads
+                    // are issued: with the residual loads issued alongside, the first operand stage landed ~10 k
+                    // cycles after griddepcontrol.wait instead of ~3 k (H100, layers 1-4 conv3)
+                    if (kTmaEpi && tile == (int)blockIdx.x && kb == min(p.num_k_blocks, kStages) - 1) mbar_arrive(res_go);
                 }
             }
             // release the dependent launch once this CTA's last operand loads are issued: an earlier release lets the
             // next kernel's CTAs sit in griddepcontrol.wait on SMs the other stream's chain could be using
             asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
             if (tr) { tr[3] = gtimer(); tr[11] = clock64(); }
+        }
+    } else if (kTmaEpi && warp > kProducerWarp) {
+        // ===================== residual producer of warpgroup g (warps 9, 10) =====================
+        // Loads the warpgroup's residual chunks in (tile, chunk) order into its ring as soon as a slot is empty, so
+        // the next tile's chunks stream in under this tile's last chunks and the next main loop.  Every chunk of
+        // every tile is loaded, also rows past M and columns past Cout (zero-filled, still counted in the bytes), so
+        // that both sides step through the ring alike.
+        if (lane == 0) {
+            const int g = warp - kProducerWarp - 1;
+            int slot = 0;
+            uint32_t sphase = 0;
+            mbar_wait(res_go, 0);
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+                const int mt = tile / p.num_n_tiles, nt = tile - mt * p.num_n_tiles;
+                for (int c = 0; c < kChunks; ++c) {
+                    uint64_t* bar = &slot_full[g * kSlots + slot];
+                    mbar_wait(&slot_empty[g * kSlots + slot], sphase ^ 1);
+                    mbar_expect_tx(bar, kEpiBox);
+                    tma_load_2d(&map_r, bar, epi + (g * kSlots + slot) * kSlotBytes, nt * BLOCK_N + 32 * c,
+                                mt * BLOCK_M + 64 * g);
+                    if (++slot == kSlots) { slot = 0; sphase ^= 1; }
+                }
+            }
         }
     } else if (STEM && warp > kProducerWarp) {
         // ===================== stem patch gather =====================
@@ -313,7 +336,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         const int out_mode = d.out_mode;
         const bool res_biased = d.res_biased != 0;
         int stage = 0;
-        uint32_t phase = 0, rphase = 0;
+        uint32_t phase = 0;
+        // epilogue ring (kTmaEpi): the next slot and its phase, and the slot of the previous tile's last chunk, whose
+        // stores may still be reading it (-1: none)
+        int slot = 0, held = -1;
+        uint32_t sphase = 0;
+        const bool store_thread = (threadIdx.x & 127) == 0;
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             const int mt = tile / p.num_n_tiles, nt = tile - mt * p.num_n_tiles;
             int prev = 0;
@@ -336,6 +364,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                 if (kb > 0 && lane == 0) mbar_arrive(&empty[prev]);
                 prev = stage;
                 if (++stage == kStages) { stage = 0; phase ^= 1; }
+                if (kTmaEpi && held >= 0) {
+                    // the previous tile's last chunk, stored at the end of its epilogue, is released here, under
+                    // this tile's first MMAs, instead of stalling that epilogue on its read
+                    if (store_thread) {
+                        bulk_wait_read<0>();
+                        mbar_arrive(&slot_empty[wg * kSlots + held]);
+                    }
+                    held = -1;
+                }
             }
             wgmma_wait<0>();
 #pragma unroll
@@ -343,57 +380,62 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             if (lane == 0) mbar_arrive(&empty[prev]);
 
             if constexpr (kTmaEpi) {
-                // ---- residual epilogue through shared memory.  The producer has loaded this warpgroup's 64 residual
-                // rows into its fp32 boxes; every thread adds its accumulator pairs to them in place and writes the
-                // fp16 twin beside them, then one thread stores the boxes by TMA (rows past M and columns past Cout
-                // are clipped) and hands the buffer back once the stores have read it.  The global writes drain
-                // while the warpgroup runs the next tile's MMAs.
+                // ---- residual epilogue through the warpgroup's ring, one 32-column chunk at a time.  The residual
+                // producer has loaded the chunk's 64 residual rows into the slot's fp32 box; every thread adds its
+                // accumulator pairs to them in place and writes the fp16 twin beside them, then one thread stores
+                // both boxes by TMA (rows past M and columns past Cout are clipped) as one bulk group.  The slot of
+                // the chunk before is handed back once its group has read it, so the warpgroup goes straight on to
+                // the next chunk and the global writes drain under the next chunks and the next tile's MMAs.
                 const int rl = 16 * (warp & 3) + (lane >> 2);     // rows rl and rl + 8 of the warpgroup's 64
-                const uint32_t rbuf = smem_u32(epi) + wg * kResWg;
-                const uint32_t tbuf = smem_u32(epi) + 2 * kResWg + wg * kTwinWg;
-                mbar_wait(&res_full[wg], rphase);
-                rphase ^= 1;
+                const int row0 = mt * BLOCK_M + 64 * wg;
 #pragma unroll
-                for (int j = 0; j < BLOCK_N / 8; ++j) {
-                    const int cl = 8 * j + cq;                    // column in the tile
-                    const int c = nt * BLOCK_N + cl;
-                    const int cs = c < d.Cout ? c : 0;            // past Cout: any in-bounds column, never stored
-                    const float2 sc = d.scale ? __ldg(reinterpret_cast<const float2*>(d.scale + cs)) : make_float2(1.f, 1.f);
-                    const float2 sh = d.shift ? __ldg(reinterpret_cast<const float2*>(d.shift + cs)) : make_float2(0.f, 0.f);
+                for (int ch = 0; ch < kChunks; ++ch) {
+                    const uint32_t rbuf = smem_u32(epi) + (wg * kSlots + slot) * kSlotBytes, tbuf = rbuf + kEpiBox;
+                    mbar_wait(&slot_full[wg * kSlots + slot], sphase);
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const uint32_t row = (uint32_t)(rl + 8 * h) * 128;
-                        const uint32_t ra = rbuf + (cl >> 5) * kEpiBox + swz128(row + (cl & 31) * 4);
-                        float2 r = lds64f(ra);
-                        float x0 = fmaf(acc[4 * j + 2 * h], sc.x, sh.x);
-                        float x1 = fmaf(acc[4 * j + 2 * h + 1], sc.y, sh.y);
-                        if (res_biased) { r.x = sb_unbias_tf32(r.x); r.y = sb_unbias_tf32(r.y); }
-                        x0 += r.x; x1 += r.y;
-                        if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-                        if (out_mode == 1) { x0 = sb_round_tf32(x0); x1 = sb_round_tf32(x1); }
-                        else if (out_mode == 2) { x0 = sb_bias_tf32(x0); x1 = sb_bias_tf32(x1); }
-                        sts64f(ra, x0, x1);
-                        if (d.out16) {   // fp16 twin (round to nearest) for the next tensor-core consumer
-                            if (out_mode == 2) { x0 = sb_unbias_tf32(x0); x1 = sb_unbias_tf32(x1); }
-                            const __half2 hv = __floats2half2_rn(x0, x1);
-                            sts32u(tbuf + (cl >> 6) * kEpiBox + swz128(row + (cl & 63) * 2),
-                                   *reinterpret_cast<const uint32_t*>(&hv));
+                    for (int jj = 0; jj < 4; ++jj) {
+                        const int j = 4 * ch + jj;
+                        const int cl = 8 * j + cq;                // column in the tile
+                        const int c = nt * BLOCK_N + cl;
+                        const int cs = c < d.Cout ? c : 0;        // past Cout: any in-bounds column, never stored
+                        const float2 sc = d.scale ? __ldg(reinterpret_cast<const float2*>(d.scale + cs)) : make_float2(1.f, 1.f);
+                        const float2 sh = d.shift ? __ldg(reinterpret_cast<const float2*>(d.shift + cs)) : make_float2(0.f, 0.f);
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const uint32_t row = (uint32_t)(rl + 8 * h);
+                            const uint32_t ra = rbuf + swz128(row * 128 + (cl & 31) * 4);
+                            float2 r = lds64f(ra);
+                            float x0 = fmaf(acc[4 * j + 2 * h], sc.x, sh.x);
+                            float x1 = fmaf(acc[4 * j + 2 * h + 1], sc.y, sh.y);
+                            if (res_biased) { r.x = sb_unbias_tf32(r.x); r.y = sb_unbias_tf32(r.y); }
+                            x0 += r.x; x1 += r.y;
+                            if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+                            if (out_mode == 1) { x0 = sb_round_tf32(x0); x1 = sb_round_tf32(x1); }
+                            else if (out_mode == 2) { x0 = sb_bias_tf32(x0); x1 = sb_bias_tf32(x1); }
+                            sts64f(ra, x0, x1);
+                            if (d.out16) {   // fp16 twin (round to nearest) for the next tensor-core consumer
+                                if (out_mode == 2) { x0 = sb_unbias_tf32(x0); x1 = sb_unbias_tf32(x1); }
+                                const __half2 hv = __floats2half2_rn(x0, x1);
+                                sts32u(tbuf + swz64(row * 64 + (cl & 31) * 2), *reinterpret_cast<const uint32_t*>(&hv));
+                            }
                         }
                     }
-                }
-                fence_proxy_async();                  // generic-proxy writes -> visible to the TMA stores
-                named_bar_sync(1 + wg, 128);
-                if ((threadIdx.x & 127) == 0) {
-                    const int row0 = mt * BLOCK_M + 64 * wg, col0 = nt * BLOCK_N;
-                    if (row0 < p.M) {
-                        for (int b = 0; d.out && b < BLOCK_N / 32; ++b)
-                            if (col0 + 32 * b < d.Cout) tma_store_2d(&map_o, rbuf + b * kEpiBox, col0 + 32 * b, row0);
-                        for (int b = 0; d.out16 && b < (BLOCK_N + 63) / 64; ++b)
-                            if (col0 + 64 * b < d.Cout) tma_store_2d(&map_o16, tbuf + b * kEpiBox, col0 + 64 * b, row0);
+                    fence_proxy_async();                  // generic-proxy writes -> visible to the TMA stores
+                    named_bar_sync(1 + wg, 128);
+                    if (store_thread) {
+                        const int col = nt * BLOCK_N + 32 * ch;
+                        if (row0 < p.M && col < d.Cout) {
+                            if (d.out) tma_store_2d(&map_o, rbuf, col, row0);
+                            if (d.out16) tma_store_2d(&map_o16, tbuf, col, row0);
+                        }
+                        bulk_commit();                    // one group per chunk, empty or not
+                        if (ch > 0) {
+                            bulk_wait_read<1>();          // all groups but this chunk's have read their slots
+                            mbar_arrive(&slot_empty[wg * kSlots + held]);
+                        }
                     }
-                    bulk_commit();
-                    bulk_wait_read<0>();
-                    mbar_arrive(&res_empty[wg]);
+                    held = slot;
+                    if (++slot == kSlots) { slot = 0; sphase ^= 1; }
                 }
             } else {
                 // ---- epilogue from registers: per row {output offset, residual row, upsample source + weights}, then
@@ -524,12 +566,12 @@ EncodeTiledFn get_encode() {
 }
 
 bool make_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-              const cuuint32_t* box, bool f16) {
+              const cuuint32_t* box, bool f16, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
     EncodeTiledFn enc = get_encode();
     if (!enc) return false;
     cuuint32_t estr[5] = {1, 1, 1, 1, 1};
     CUresult r = enc(m, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<void*>(base), dims,
-                     strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                     strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS;
 }
@@ -592,7 +634,8 @@ struct TcMaps {
 
 template <int BN, int ST, bool RES, bool UP, bool IN16, bool STEM = false, bool MASK = false>
 int launch_t(const TcMaps& m, const TcParams& p, cudaStream_t st) {
-    constexpr size_t smem = conv_smem(BN, ST, tma_epilogue(RES, IN16, MASK) ? epi_bytes(BN) : 0);
+    constexpr bool tma_epi = tma_epilogue(RES, IN16, MASK);
+    constexpr size_t smem = conv_smem(BN, ST, tma_epi ? epi_slots(BN) : 0);
     static_assert(smem <= 227 * 1024, "smem budget");
     auto kern = conv_tc_kernel<BN, ST, RES, UP, IN16, STEM, MASK>;
     static bool attr_done[kSbMaxDevices] = {false};
@@ -608,7 +651,7 @@ int launch_t(const TcMaps& m, const TcParams& p, cudaStream_t st) {
     const int grid = tiles < slots ? tiles : slots;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(STEM ? kStemThreads : kThreads);
+    cfg.blockDim = dim3(conv_threads(STEM, tma_epi));
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
     cudaLaunchAttribute attrs[1];
@@ -623,7 +666,7 @@ int launch_t(const TcMaps& m, const TcParams& p, cudaStream_t st) {
     return SB_OK;
 }
 
-// ST: operand stages; ST_RES: operand stages beside the TMA residual epilogue's buffers (0: no such variant)
+// ST: operand stages; ST_RES: operand stages beside the TMA residual epilogue's rings (0: no such variant)
 template <int BN, int ST, int ST_RES>
 int launch(const TcMaps& m, const TcParams& p, bool dgrad, cudaStream_t st) {
     const bool res = p.d.residual != nullptr, up = p.d.up_src != nullptr;   // never both (supported())
@@ -777,22 +820,22 @@ int conv2d_tc(const sb_conv_desc* d, const __half* mask16, bool dgrad, bool rows
         if (!make_map(&mb, d->wgt, 2, dims, strides, box, f16)) return SB_EINVAL;
     }
     if (d->residual && f16 && !dgrad) {
-        // TMA residual epilogue: [Cout, M] boxes of 64 rows, 32 fp32 / 64 fp16 columns.  A 32-wide tile (Cout <= 32)
-        // stores its twin through a 64-column box whose upper half lies past Cout and is clipped.
+        // TMA residual epilogue: [Cout, M] boxes of 64 rows and 32 columns, one ring chunk each; the fp16 box has
+        // 64-byte rows, so it is 64-byte swizzled
         const cuuint64_t dims[2] = {(cuuint64_t)d->Cout, (cuuint64_t)p.M};
-        const cuuint32_t box32[2] = {32, 64}, box16[2] = {64, 64};
+        const cuuint32_t box32[2] = {32, 64};
         const cuuint64_t rs[1] = {(cuuint64_t)d->res_ld * 4};
         if (!make_map(&m.r, d->residual, 2, dims, rs, box32, false)) return SB_EINVAL;
         const cuuint64_t os[1] = {(cuuint64_t)d->out_w_stride * 4}, os16[1] = {(cuuint64_t)d->out_w_stride * 2};
         if (d->out && !make_map(&m.o, d->out + d->out_coff, 2, dims, os, box32, false)) return SB_EINVAL;
         if (d->out16 && !make_map(&m.o16, reinterpret_cast<const __half*>(d->out16) + d->out_coff, 2, dims, os16,
-                                  box16, true))
+                                  box32, true, CU_TENSOR_MAP_SWIZZLE_64B))
             return SB_EINVAL;
     }
     cudaStream_t st = sb_cs(stream);
-    switch (BN) {        // <BN, operand stages, operand stages beside the residual epilogue buffers>
-        case 32: return launch<32, 9, 9>(m, p, dgrad, st);
-        case 64: return launch<64, 8, 7>(m, p, dgrad, st);
+    switch (BN) {        // <BN, operand stages, operand stages beside the residual epilogue rings>
+        case 32: return launch<32, 9, 7>(m, p, dgrad, st);
+        case 64: return launch<64, 8, 6>(m, p, dgrad, st);
         case 256: return launch<256, 4, 0>(m, p, dgrad, st);
         default: return launch<128, 6, 4>(m, p, dgrad, st);
     }

@@ -129,5 +129,7 @@ __device__ __forceinline__ void sts32u(uint32_t saddr, uint32_t v) {
 // byte offset inside a 1024-byte-aligned region written / read by TMA with 128-byte swizzle: 16-byte chunk
 // (bits 4..6) XOR 128-byte row (bits 7..9)
 __device__ __forceinline__ uint32_t swz128(uint32_t off) { return off ^ (((off >> 7) & 7u) << 4); }
+// the same with 64-byte swizzle (512-byte aligned region): 16-byte chunk (bits 4..5) XOR bits 7..8
+__device__ __forceinline__ uint32_t swz64(uint32_t off) { return off ^ (((off >> 7) & 3u) << 4); }
 
 }  // namespace
