@@ -589,7 +589,7 @@ int sb_pack_weights(const sb_pack_target* targets, const sb_pack_target* targets
  *   the mirrored frames.
  * sb_train_gt -- the ground truth of a step (minibatch.py:43-85, roibatchLoader.py:72-107) for B images, one CTA per
  *   image.  Inputs are the roidb rows of each image at a fixed capacity N <= 1024: boxes_left / boxes_right /
- *   boxes_merge [B,N,4], gt_classes [B,N] int32, dim_orien [B,N,4] (h, w, l, theta), kpts [B,N,6], n_rows [B] int32
+ *   boxes_merge [B,N,4], gt_classes [B,N] int32, dim_orien [B,N,4] (w, h, l, alpha), kpts [B,N,6], n_rows [B] int32
  *   on the DEVICE (rows in use, clamped to [0, N] by the kernel) and words [B,N] uint32.  Rows with gt_classes == 0
  *   are dropped; boxes and keypoints are multiplied by im_scale in fp32 (a float32 array times a Python float);
  *   x1 = min(x1, im_width); (sin, cos) of theta are evaluated in fp64 and rounded (math.sin of a float32); a scaled
@@ -649,6 +649,37 @@ int sb_kitti_eval(const double* gt, const int* gt_code, const double* det, const
                   void* workspace, size_t workspace_bytes, double* thresholds, int* n_thresholds, long long* tp,
                   long long* fp, long long* fn, double* sim, double* precision, double* recall, double* aos,
                   double* ap, long long* n_gt, sb_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * The training ground truth of a KITTI split (the reference's gt_roidb, DESIGN.md §10): kitti_utils.read_obj_data,
+ * kitti.remove_occluded_keypoints for the left and then the right camera, and _load_kitti_annotation's filter.
+ *
+ * Rows: SB_KITTI_ANN_IN doubles per label line of type Car, Van, Truck or Misc (every other line is left out by the
+ * caller) -- trunc, occ, alpha, w, h, l, x, y, z, cos(ry + pi/2), sin(ry + pi/2) -- and an int32 code per row: 0 Car,
+ * 1 another of those types.  The rows of image i are obj_off[i] .. obj_off[i+1] in label order (int64 offsets in
+ * DEVICE memory, obj_off[0] = 0; no cap per image).  calib: SB_KITTI_ANN_CALIB doubles per image in DEVICE memory --
+ * p2_2 (P2 with [0,3] = 0), p2_3 (P3 with [0,3] = P3[0,3] - P2[0,3]), both 3x4 row-major, then t = (P2[0,3] -
+ * P0[0,3]) / P2[0,0]; image_hw: int32 [n_images, 2] (H, W of the left image) in DEVICE memory.
+ * sb_kitti_annotations -- one CTA per image, fp64 throughout.  Outputs: the kept rows of image i, in label order, at
+ *   rows obj_off[i] .. obj_off[i] + n_kept[i] of out (float32 [n_rows, SB_KITTI_ANN_OUT]: boxes_left[4],
+ *   boxes_right[4], boxes_merge[4], dim_orien[4] = (w, h, l, alpha), kpts[6] = (4 keypoints, visible left, visible
+ *   right) of the left camera, kpts_right[6] of the right camera, truncation, occlusion), zeros in the image's other
+ *   rows; n_kept [n_images] int32; status [n_images] int32: 0, 1 + the index (within the image's rows) of the object
+ *   the reference indexes the SB_KITTI_DEPTH_COLS-column depth line out of range with (it raises IndexError there;
+ *   nothing is kept) -- the first whose painted columns int(x1) .. int(x2) reach past the line, else the first with
+ *   int(x1) or int(x2) past it -- or -1 for an image whose H or W is not positive (nothing is kept).  The workspace is 256-byte
+ *   aligned and at least sb_kitti_annotations_workspace_bytes (0 for sizes it refuses).
+ * SB_EINVAL before any launch for a null pointer, n_images < 1, a negative row count or a workspace that is too small
+ *   or misaligned.                                                                                                 */
+#define SB_KITTI_ANN_IN 11
+#define SB_KITTI_ANN_OUT 30
+#define SB_KITTI_ANN_CALIB 25
+#define SB_KITTI_DEPTH_COLS 1260
+
+size_t sb_kitti_annotations_workspace_bytes(int n_images, long long n_rows);
+int sb_kitti_annotations(const double* rows, const int* codes, const long long* obj_off, const double* calib,
+                         const int* image_hw, int n_images, long long n_rows, void* workspace,
+                         size_t workspace_bytes, float* out, int* n_kept, int* status, sb_stream_t stream);
 
 #ifdef __cplusplus
 }

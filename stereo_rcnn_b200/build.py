@@ -12,7 +12,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libstereo_b200.so")
 SOURCES = ["misc.cu", "nms.cu", "proposal.cu", "roi_align.cu", "dense_align.cu", "conv_simt.cu", "conv_tc.cu", "conv_wgrad.cu", "peer.cu", "box_solver.cu",
-           "train_targets.cu", "train_loss.cu", "heads_bwd.cu", "optim.cu", "train_input.cu", "kitti_eval.cu"]
+           "train_targets.cu", "train_loss.cu", "heads_bwd.cu", "optim.cu", "train_input.cu", "kitti_eval.cu",
+           "kitti_annotations.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
          "-Xcompiler", "-Wall", "-Xcompiler", "-Wno-unused-function"]

@@ -184,6 +184,9 @@ _SIGS = {
     "sb_kitti_eval_workspace_bytes": (c_size_t, [c_int, c_ll, c_ll, c_ll, c_int]),
     "sb_kitti_eval": (c_int, [c_void_p] * 7 + [c_int, c_ll, c_ll, c_ll, ctypes.POINTER(c_double), c_int, c_void_p,
                               c_size_t] + [c_void_p] * 11 + [c_void_p]),
+    # the training ground truth of a KITTI split
+    "sb_kitti_annotations_workspace_bytes": (c_size_t, [c_int, c_ll]),
+    "sb_kitti_annotations": (c_int, [c_void_p] * 5 + [c_int, c_ll, c_void_p, c_size_t] + [c_void_p] * 3 + [c_void_p]),
 }
 
 EXPORTS = tuple(_SIGS)

@@ -940,6 +940,36 @@ def kitti_eval(gt, gt_code, det, det_code, gt_off, det_off, pair_off, n_pairs, b
     return out
 
 
+KITTI_ANN_IN, KITTI_ANN_OUT, KITTI_ANN_CALIB, KITTI_DEPTH_COLS = 11, 30, 25, 1260  # the SB_KITTI_ANN_* constants
+
+
+def kitti_annotations(rows, codes, obj_off, calib, image_hw, out=None):
+    """sb_kitti_annotations over a packed split: rows fp64 [n,11], codes int32 [n], obj_off int64 [n_images+1], calib
+    fp64 [n_images,25], image_hw int32 [n_images,2], all on the device -> (out fp32 [n,30], n_kept int32 [n_images],
+    status int32 [n_images]); out: those three tensors to write into"""
+    L = _l.load()
+    n_images, n = obj_off.numel() - 1, codes.numel()
+    dev = obj_off.device
+    assert rows.dtype == torch.float64 and codes.dtype == torch.int32 and obj_off.dtype == torch.int64
+    assert calib.dtype == torch.float64 and image_hw.dtype == torch.int32
+    assert rows.numel() == n * KITTI_ANN_IN and calib.numel() == n_images * KITTI_ANN_CALIB
+    assert image_hw.numel() == 2 * n_images
+    nb = L.sb_kitti_annotations_workspace_bytes(n_images, n)
+    if nb == 0:
+        raise ValueError("sb_kitti_annotations refuses these sizes (%d images, %d rows)" % (n_images, n))
+    ws = workspace(nb + 256, dev, "kitti_annotations")
+    base = (-ws.data_ptr()) % 256
+    if out is None:
+        out = (torch.empty(max(n, 1), KITTI_ANN_OUT, dtype=torch.float32, device=dev)[:n],
+               torch.empty(n_images, dtype=torch.int32, device=dev), torch.empty(n_images, dtype=torch.int32, device=dev))
+    assert out[0].shape == (n, KITTI_ANN_OUT) and out[1].numel() == out[2].numel() == n_images
+    check(L.sb_kitti_annotations(ptr(rows) if n else None, ptr(codes) if n else None, ptr(obj_off), ptr(calib),
+                                 ptr(image_hw), n_images, n, ctypes.c_void_p(ws.data_ptr() + base), nb,
+                                 ptr(out[0]) if n else None, ptr(out[1]), ptr(out[2]), stream_ptr()),
+          "sb_kitti_annotations")
+    return out
+
+
 def kitti_eval_outputs(n_bars, device):
     """the output tensors of kitti_eval for n_bars bars: views into one device buffer (one D2H copies them all)"""
     C = 9 * n_bars

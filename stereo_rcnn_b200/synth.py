@@ -308,3 +308,61 @@ def kitti_split(n_images, seed=0, n_cars=4, n_dets=30):
             dets.append(line(k, r, rs.uniform(0.05, 1.0)))
         split.append(("".join(labels), "".join(dets)))
     return split
+
+
+def png_bytes(rgb):
+    """a uint8 [H,W,3] array as an 8-bit RGB PNG file (zlib, no filter)"""
+    import struct
+    a = np.ascontiguousarray(rgb, np.uint8)
+    h, w = a.shape[:2]
+
+    def chunk(tag, data):
+        return struct.pack(">I", len(data)) + tag + data + struct.pack(">I", zlib.crc32(tag + data) & 0xFFFFFFFF)
+    raw = b"".join(b"\x00" + a[r].tobytes() for r in range(h))
+    return (b"\x89PNG\r\n\x1a\n" + chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, 8, 2, 0, 0, 0)) +
+            chunk(b"IDAT", zlib.compress(raw, 1)) + chunk(b"IEND", b""))
+
+
+def kitti_folder(root, n_images, seed=0, sizes=((375, 1242), (370, 1224)), frames=None):
+    """A seeded synthetic KITTI training folder: root/training/label_2 (kitti_split's label texts), calib (KITTI-like
+    P0-P3 around the demo calibration) and image_2 / image_3.  The images are PNG headers only (enough for
+    kitti_data, which reads the size) unless frames(k) -> (left, right) uint8 [H,W,3] gives the pixels; image k has
+    size sizes[k % len(sizes)].  -> the image ids"""
+    import os
+    rs = np.random.RandomState(seed + 1)
+    d = os.path.join(root, "training")
+    for sub in ("label_2", "calib", "image_2", "image_3"):
+        os.makedirs(os.path.join(d, sub), exist_ok=True)
+    ids = []
+    for k, (labels, _dets) in enumerate(kitti_split(n_images, seed)):
+        i = "%06d" % k
+        ids.append(i)
+        f = DEMO_P2[0, 0] + rs.uniform(-15, 15)
+        cx, cy = DEMO_P2[0, 2] + rs.uniform(-8, 8), DEMO_P2[1, 2] + rs.uniform(-8, 8)
+        rows = []
+        for name, t in (("P0", (0.0, 0.0, 0.0)), ("P1", (-f * 0.54, 0.0, 0.0)),
+                        ("P2", (DEMO_P2[0, 3] + rs.uniform(-1, 1), DEMO_P2[1, 3], DEMO_P2[2, 3])),
+                        ("P3", (DEMO_P3[0, 3] + rs.uniform(-3, 3), DEMO_P3[1, 3], DEMO_P3[2, 3]))):
+            rows.append("%s: %s" % (name, " ".join("%.12e" % v for v in (f, 0.0, cx, t[0], 0.0, f, cy, t[1], 0.0, 0.0,
+                                                                        1.0, t[2]))))
+        rows += ["R0_rect: " + " ".join(["1.0", "0.0", "0.0", "0.0", "1.0", "0.0", "0.0", "0.0", "1.0"]),
+                 "Tr_velo_to_cam: " + " ".join(["0.0"] * 12), "Tr_imu_to_velo: " + " ".join(["0.0"] * 12)]
+        h, w = sizes[k % len(sizes)]
+        # objects in view only, as in KITTI's labels (one whose box starts past the depth line is refused)
+        labels = "".join(l + "\n" for l in labels.splitlines() if l.startswith("DontCare") or
+                         (float(l.split()[4]) > 0.0 and float(l.split()[6]) < w - 1))
+        with open(os.path.join(d, "label_2", i + ".txt"), "w") as fh:
+            fh.write(labels)
+        with open(os.path.join(d, "calib", i + ".txt"), "w") as fh:
+            fh.write("\n".join(rows) + "\n\n")
+        if frames is not None:
+            pair = frames(k)
+            assert pair[0].shape[:2] == (h, w)
+        for j, sub in enumerate(("image_2", "image_3")):
+            with open(os.path.join(d, sub, i + ".png"), "wb") as fh:
+                if frames is not None:
+                    fh.write(png_bytes(pair[j]))
+                else:
+                    fh.write(png_bytes(np.zeros((1, 1, 3), np.uint8))[:16] + w.to_bytes(4, "big") +
+                             h.to_bytes(4, "big") + b"\x08\x02\x00\x00\x00")
+    return ids
