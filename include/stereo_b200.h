@@ -538,7 +538,7 @@ int sb_clip_gradient(float* const* grads, const size_t* counts, int n_tensors, f
  *       v = src[src_offset + sum_k i_k src_stride[k]]                    (strides may be negative: a tap flip)
  *       dst[dst_offset + sum_k i_k dst_stride[k]] = T(v);  dst16[same] = (half)v when dst16 != NULL
  *   with T one of SB_PACK_F32 (copy), SB_PACK_TF32 (round to TF32, nearest with ties away: (bits + 0x1000) & ~0x1fff,
- *   the integer rounding of the engine's host packing), SB_PACK_F16 (fp16, round to nearest even) and
+ *   the integer rounding of ops.round_tf32_), SB_PACK_F16 (fp16, round to nearest even) and
  *   SB_PACK_SCALE_F16 (fp16 of the fp32 product v * scale[i_{scale_dim}]).  dst is fp32 for the first two, fp16 for
  *   the others; dst16 (an fp16 twin with dst's strides) is allowed with the fp32 transforms only.  dst_stride[3] must be
  *   1.  A target whose src_stride[3] != 1 is transposed through shared memory in tiles of up to 288 (i1, i2) rows x 32

@@ -19,11 +19,6 @@ STRIDES = [1, 2, 2, 2]
 EPS = 1e-5
 
 
-def _pack_conv(w):
-    """[Cout,Cin,kh,kw] -> [Cout,kh,kw,Cin] contiguous (K-major rows, one per output channel)"""
-    return w.permute(0, 2, 3, 1).contiguous()
-
-
 def trainable_trunk_fpn_params(fixed_blocks=1):
     """[(name, shape)] of the trunk + FPN parameters that receive a gradient (resnet.py:289-309 of the reference):
     RCNN_layer0 and every BatchNorm are frozen, cfg.RESNET.FIXED_BLOCKS = k also freezes RCNN_layer1..k, the FPN convs
@@ -105,22 +100,30 @@ class RpnSaved(object):
 
 
 _LEVELS = ("p2", "p3", "p4", "p5", "p6")
+_FC = ("RCNN_cls_score.weight", "RCNN_cls_score.bias", "RCNN_bbox_pred.weight", "RCNN_bbox_pred.bias",
+       "RCNN_dim_orien_pred.weight", "RCNN_dim_orien_pred.bias")
 
 
 # which lateral conv reads the input of RCNN_layer<li+1> (li = 1..3): c2 -> latlayer3, c3 -> latlayer2, c4 -> latlayer1
 _LATERAL_OF_INPUT = {1: ("RCNN_latlayer3", "dt2"), 2: ("RCNN_latlayer2", "dt3"), 3: ("RCNN_latlayer1", "dt4")}
 
 
+def _alloc(shape, dtype, device, zeroed=False):
+    """a device tensor for sb_pack_weights to fill; zeroed ones (padding the table never writes) are host zeros
+    copied over, so that building an engine launches no torch kernel"""
+    if zeroed:
+        return torch.zeros(shape, dtype=dtype).to(device)
+    return torch.empty(shape, dtype=dtype, device=device)
+
+
 class _DgradConv(object):
-    """conv weights for the data gradient: [Cin][kh][kw][Cout] fp16, taps flipped, frozen-BN scale folded in"""
+    """conv weights for the data gradient (the forward conv Cin -> Cout run backwards, Cout -> Cin here):
+    w16 [Cout][kh][kw][Cin] fp16, written by sb_pack_weights (StereoRCNNEngine._pack_targets)"""
     __slots__ = ("w16", "Cin", "Cout", "kh", "kw", "pad")
 
-    def __init__(self, w, scale, pad, device):
-        co, ci, self.kh, self.kw = w.shape
-        if scale is not None:
-            w = w * scale.view(-1, 1, 1, 1)
-        self.w16 = w.flip(2, 3).permute(1, 2, 3, 0).contiguous().to(torch.float16).to(device)
-        self.Cin, self.Cout, self.pad = co, ci, pad
+    def __init__(self, Cin, Cout, kh, kw, pad, device, zeroed=False):
+        self.Cin, self.Cout, self.kh, self.kw, self.pad = Cin, Cout, kh, kw, pad
+        self.w16 = _alloc((Cout, kh, kw, Cin), torch.float16, device, zeroed)
 
 
 def _numel(shape):
@@ -152,18 +155,16 @@ class _PackT(object):
 
 
 class PackedConv(object):
+    """a forward conv on the device: w [Cout][kh][kw][Cin] fp32 and, in fp16 engines, its fp16 twin w16, written by
+    sb_pack_weights (StereoRCNNEngine._pack_targets); scale the folded frozen-BN scale (None for a conv with a bias),
+    shift the folded BN shift or the bias"""
     __slots__ = ("w", "w16", "scale", "shift", "Cin", "Cout", "kh", "kw", "pad")
 
-    round_weights = True      # class-wide switch: False keeps exact fp32 weights (SIMT yardstick runs)
-    make_half = False         # class-wide switch: also keep an fp16 copy (fp16-operand mode)
-
-    def __init__(self, w, scale, shift, pad):
-        self.Cout, self.Cin, self.kh, self.kw = w.shape
-        wp = _pack_conv(w).clone()
-        self.w16 = wp.to(torch.float16) if PackedConv.make_half else None    # f16 operand (round to nearest)
-        if PackedConv.round_weights:   # round to TF32 (nearest) once: the tensor core would otherwise truncate
-            ops.round_tf32_(wp)
-        self.w, self.scale, self.shift, self.pad = wp, scale, shift, pad
+    def __init__(self, Cout, Cin, kh, kw, pad, scale, shift, half, device, zeroed=False):
+        self.Cout, self.Cin, self.kh, self.kw, self.pad = Cout, Cin, kh, kw, pad
+        self.w = _alloc((Cout, kh, kw, Cin), torch.float32, device, zeroed)
+        self.w16 = _alloc((Cout, kh, kw, Cin), torch.float16, device, zeroed) if half else None
+        self.scale, self.shift = scale, shift
 
 
 class StereoRCNNEngine(object):
@@ -192,91 +193,61 @@ class StereoRCNNEngine(object):
         self.record = None        # bench: list collecting (desc, live tensors) of every conv launch of a forward
         # conv_impl="simt" is the exact-fp32 yardstick: exact weights, exact stores, no TF32 hygiene modes
         self.exact = conv_impl == "simt"
-        PackedConv.round_weights = not self.exact
-        PackedConv.make_half = self.half
-        # Weights are folded and packed ON THE HOST (one-off, ~1 s) and reach the device by plain copies: no torch
-        # kernel runs on the GPU for it, so a profiler's launch window of a process that builds an engine shows this
-        # library's kernels, not ~950 elementwise launches of weight preparation.
-        sd = {k: v.detach().to("cpu", torch.float32) for k, v in state_dict.items()
+        # The BN fold is host arithmetic on frozen values; every weight layout is written by one sb_pack_weights launch
+        # over the table of _pack_targets, from fp32 masters uploaded by plain copies and dropped after: no torch kernel
+        # runs on the GPU for it, so a profiler's launch window of a process that builds an engine shows this library's
+        # kernels only.  The host masters stay for the data-gradient copies, packed on first use.
+        sd = {k: v.detach().to("cpu", torch.float32).contiguous() for k, v in state_dict.items()
               if not k.endswith("num_batches_tracked")}
-        self.p = {}
-        # exact host weights and BN scales of the trunk + FPN convs, for the backward's transposed weights (packed on
-        # the device only when a backward is first requested)
-        self._bwd_src = {}
+        self._masters = sd
+        self._trainable = dict(trainable_trunk_fpn_params(0) + trainable_rpn_params() +
+                               trainable_rcnn_head_params(n_classes))
         self._bwd = None
         self._found_inf = None
+        dev, h = self.device, self.half
+        empty = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)
+        self.p = {}
 
         def bn_fold(k):
             s = sd[k + ".weight"] / torch.sqrt(sd[k + ".running_var"] + EPS)
-            return s.contiguous(), (sd[k + ".bias"] - sd[k + ".running_mean"] * s).contiguous()
+            return s.to(dev), (sd[k + ".bias"] - sd[k + ".running_mean"] * s).to(dev)
 
-        def conv_bn(ck, bk, pad):
-            s, b = bn_fold(bk)
-            self.p[ck] = PackedConv(sd[ck + ".weight"], s, b, pad)
-            if ck.startswith("RCNN_layer"):
-                self._bwd_src[ck] = (sd[ck + ".weight"], s, pad)
+        def conv(key, pad, bn=None):
+            co, ci, kh, kw = sd[key + ".weight"].shape
+            scale, shift = bn_fold(bn) if bn is not None else (None, empty(co))
+            self.p[key] = PackedConv(co, ci, kh, kw, pad, scale, shift, h, dev)
 
-        def conv_bias(ck, pad):
-            self.p[ck] = PackedConv(sd[ck + ".weight"], None, sd[ck + ".bias"].contiguous(), pad)
-            self._bwd_src[ck] = (sd[ck + ".weight"], None, pad)
-
-        # stem: [64,3,7,7] -> [64][7][7][3]
         s, b = bn_fold("RCNN_layer0.1")
-        self.stem = (_pack_conv(sd["RCNN_layer0.0.weight"]), s, b)
-        wst = torch.zeros(64, 160, 1, 1)                              # stem as a GEMM over the padded patch matrix
-        wst[:, :147, 0, 0] = sd["RCNN_layer0.0.weight"].reshape(64, 147)      # (ci, r, s) order of sb_stem_im2col
-        self.p["stem_gemm"] = PackedConv(wst, s, b, 0)
-        self.stem_w16 = ops.pack_stem_w16(sd["RCNN_layer0.0.weight"])   # K layout of the fused (implicit-GEMM) stem
+        self.stem = (empty(64, 7, 7, 3), s, b)
+        # the stem as a GEMM over sb_stem_im2col's patch matrix (K = 147 taps padded to 160), and the fp16 K layout of
+        # the fused stem sb_stem_conv_tc (padded to three 64-wide K-steps)
+        self.p["stem_gemm"] = PackedConv(64, 160, 1, 1, 0, s, b, h, dev, zeroed=True)
+        self.stem_w16 = _alloc((64, 192), torch.float16, dev, zeroed=True)
         for li, nb in enumerate(LAYERS):
             for bi in range(nb):
                 p = "RCNN_layer%d.0.%d" % (li + 1, bi)
-                conv_bn(p + ".conv1", p + ".bn1", 0)
-                conv_bn(p + ".conv2", p + ".bn2", 1)
-                conv_bn(p + ".conv3", p + ".bn3", 0)
+                conv(p + ".conv1", 0, p + ".bn1")
+                conv(p + ".conv2", 1, p + ".bn2")
+                conv(p + ".conv3", 0, p + ".bn3")
                 if bi == 0:
-                    conv_bn(p + ".downsample.0", p + ".downsample.1", 0)
+                    conv(p + ".downsample.0", 0, p + ".downsample.1")
         for k in ("RCNN_toplayer", "RCNN_latlayer1", "RCNN_latlayer2", "RCNN_latlayer3"):
-            conv_bias(k, 0)
+            conv(k, 0)
         for k in ("RCNN_smooth1", "RCNN_smooth2", "RCNN_smooth3", "RCNN_rpn.RPN_Conv"):
-            conv_bias(k, 1)
+            conv(k, 1)
         # RPN 1x1 heads fused: rows 0..5 cls logits, 6..23 box deltas, 24..31 zero padding
-        wh = torch.zeros(32, 1024, 1, 1)
-        bh = torch.zeros(32)
-        wh[0:6] = sd["RCNN_rpn.RPN_cls_score.weight"]
-        wh[6:24] = sd["RCNN_rpn.RPN_bbox_pred_left_right.weight"]
-        bh[0:6] = sd["RCNN_rpn.RPN_cls_score.bias"]
-        bh[6:24] = sd["RCNN_rpn.RPN_bbox_pred_left_right.bias"]
-        self.p["rpn_heads"] = PackedConv(wh, None, bh, 0)
-        wh64 = torch.zeros(64, 1024, 1, 1)        # the head's data gradient: K = 64 rows (rows 24..63 zero)
-        wh64[:32] = wh
-        self._bwd_src["rpn_heads"] = (wh64, None, 0)
+        self.p["rpn_heads"] = PackedConv(32, 1024, 1, 1, 0, None, _alloc(32, torch.float32, dev, True), h, dev,
+                                         zeroed=True)
         # box head: Conv2d(512,2048,k=7,s=7) on a 7x7 map == FC over (ph,pw,c) of the NHWC pooled tile
-        w0 = sd["RCNN_top.0.weight"]                                   # [2048,512,7,7]
-        self.p["RCNN_top.0"] = PackedConv(_pack_conv(w0).reshape(2048, 7 * 7 * 512, 1, 1), None,
-                                          sd["RCNN_top.0.bias"].contiguous(), 0)
-        conv_bias("RCNN_top.3", 0)
+        self.p["RCNN_top.0"] = PackedConv(2048, 7 * 7 * 512, 1, 1, 0, None, empty(2048), h, dev)
+        conv("RCNN_top.3", 0)
         for i in range(0, 12, 2):
-            conv_bias("RCNN_kpts.%d" % i, 1)
+            conv("RCNN_kpts.%d" % i, 1)
         # ConvTranspose2d(256,256,2,2): out[2i+a,2j+b] = W[:,:,a,b]^T x[i,j]  -> four 1x1 convs
-        wd = sd["RCNN_kpts.12.weight"]                                 # [Cin,Cout,2,2]
-        self.deconv = [[PackedConv(wd[:, :, a, b].t().contiguous().reshape(256, 256, 1, 1), None,
-                                   sd["RCNN_kpts.12.bias"].contiguous(), 0) for b in range(2)] for a in range(2)]
-        # host weights of the two head convs whose data gradient has its own packing (packed on the device only when
-        # heads_backward is first called): RCNN_top.0 as the forward's 1x1 conv over (ph, pw, c), and the deconv as one
-        # 1x1 conv 256 -> 1024 whose output channel (a, b, co) is phase (a, b) of output channel co
-        self._heads_bwd_src = {"RCNN_top.0": w0, "deconv": wd}
-        self.kpts_class = (sd["kpts_class.weight"].reshape(6, 256).contiguous(), sd["kpts_class.bias"].contiguous())
-        self.fc = [sd[k].contiguous() for k in ("RCNN_cls_score.weight", "RCNN_cls_score.bias",
-                                                "RCNN_bbox_pred.weight", "RCNN_bbox_pred.bias",
-                                                "RCNN_dim_orien_pred.weight", "RCNN_dim_orien_pred.bias")]
-        # ---- host -> device (copies only)
-        mv = lambda t: None if t is None else t.contiguous().to(self.device)
-        for pc in list(self.p.values()) + [c for row in self.deconv for c in row]:
-            pc.w, pc.w16, pc.scale, pc.shift = mv(pc.w), mv(pc.w16), mv(pc.scale), mv(pc.shift)
-        self.stem = tuple(mv(t) for t in self.stem)
-        self.stem_w16 = mv(self.stem_w16)
-        self.kpts_class = tuple(mv(t) for t in self.kpts_class)
-        self.fc = [mv(t) for t in self.fc]
+        self.deconv = [[PackedConv(256, 256, 1, 1, 0, None, empty(256), h, dev) for b in range(2)] for a in range(2)]
+        self.kpts_class = (empty(6, 256), empty(6))
+        self.fc = [empty(*sd[k].shape) for k in _FC]
+        self._pack_from_host(self._pack_targets()[0])
 
     # ------------------------------------------------------------------ helpers
     def _conv(self, x, pc, relu=False, stride=1, residual=None, up_src=None, out=None, out_coff=0,
@@ -444,10 +415,26 @@ class StereoRCNNEngine(object):
         return feats
 
     # ------------------------------------------------------------------ backward of the trunk + FPN
-    def _pack_backward(self):
+    def _pack_backward(self, heads=False):
+        """the data-gradient copies {key: _DgradConv}, allocated and packed from the host masters on first use: those
+        of the trunk, FPN and RPN convs, and with heads=True also the two of the R-CNN heads with their own layout"""
         if self._bwd is None:
-            self._bwd = {k: _DgradConv(w, s, pad, self.device) for k, (w, s, pad) in self._bwd_src.items()}
+            self._bwd = {}
             self._found_inf = torch.zeros(4, dtype=torch.int32, device=self.device)   # [0]; sb_fill writes 4-word units
+        dev, new = self.device, {}
+        if "rpn_heads" not in self._bwd:
+            for k, pc in self.p.items():
+                if k not in ("stem_gemm", "rpn_heads", "RCNN_top.0"):
+                    new[k] = _DgradConv(pc.Cout, pc.Cin, pc.kh, pc.kw, pc.pad, dev)
+            new["rpn_heads"] = _DgradConv(64, 1024, 1, 1, 0, dev, zeroed=True)   # K = 64 rows, 24..63 zero
+        if heads and "deconv" not in self._bwd:
+            # RCNN_top.0 as the forward's 1x1 conv over (ph, pw, c) (103 MB), and the deconv as one 1x1 conv
+            # 256 -> 1024 whose output channel (a, b, co) is phase (a, b) of output channel co
+            new["RCNN_top.0"] = _DgradConv(2048, 7 * 7 * 512, 1, 1, 0, dev)
+            new["deconv"] = _DgradConv(1024, 256, 1, 1, 0, dev)
+        if new:
+            self._bwd.update(new)
+            self._pack_from_host(self._pack_targets(new)[1])
         return self._bwd
 
     @property
@@ -732,12 +719,7 @@ class StereoRCNNEngine(object):
 
     # ------------------------------------------------------------------ backward of the R-CNN heads
     def _pack_heads_backward(self):
-        self._pack_backward()
-        if "RCNN_top.0" not in self._bwd:
-            w0, wd = self._heads_bwd_src["RCNN_top.0"], self._heads_bwd_src["deconv"]
-            self._bwd["RCNN_top.0"] = _DgradConv(_pack_conv(w0).reshape(2048, 7 * 7 * 512, 1, 1), None, 0, self.device)
-            # deconv as a 1x1 conv with output channel (a, b, co): W[(a, b, co)][ci] = wd[ci, co, a, b]
-            self._bwd["deconv"] = _DgradConv(wd.permute(2, 3, 1, 0).reshape(1024, 256, 1, 1), None, 0, self.device)
+        return self._pack_backward(heads=True)
 
     def heads_backward(self, saved, d_cls_score, d_bbox_pred, d_dim_orien_pred, d_kpts_pred, d_left_border_pred,
                        d_right_border_pred, grads=None, grad_scale=1.0, clear_found_inf=True):
@@ -828,91 +810,119 @@ class StereoRCNNEngine(object):
                                        nonfinite=self._found_inf)
         return d_feats
 
-    # ------------------------------------------------------------------ device-side refresh of the packed weights
-    def _conv_targets(self, key, name):
-        """pack targets of conv `key` from its master weight [Cout,Cin,kh,kw]: the forward's K-major copy
-        [Cout][kh][kw][Cin] (TF32-rounded fp32 plus its fp16 twin) and the data gradient's [Cin][kh][kw][Cout] fp16,
-        taps flipped, the frozen-BN scale folded in for the trunk convs"""
-        pc, bw = self.p[key], self._bwd[key]
-        co, ci, T = pc.Cout, pc.Cin, pc.kh * pc.kw
-        fw = _PackT(name, pc.w, (1, 1, 1, co * ci), (0, 0, 0, 1), (0, 0, 0, 1), self._fwd_transform, dst16=pc.w16)
-        if T > 1:       # i1 = tap, i2 = co, i3 = ci
-            fw = _PackT(name, pc.w, (1, T, co, ci), (0, 1, T * ci, T), (0, ci, T * ci, 1), self._fwd_transform,
-                        dst16=pc.w16)
-        # i1 = flipped tap t' (source tap T-1-t'), i2 = ci, i3 = co
-        scale = pc.scale if key.startswith("RCNN_layer") else None
-        dg = _PackT(name, bw.w16, (1, T, ci, co), (0, -1, T, ci * T), (0, co, T * co, 1),
-                    _lib.PACK_SCALE_F16 if scale is not None else _lib.PACK_F16, src_offset=T - 1,
-                    scale=scale)
-        return [fw, dg]
+    # ------------------------------------------------------------------ the packed weights
+    def _pack_targets(self, dgrad=()):
+        """Every packed copy of the weights, as sb_pack_targets that read the masters in the reference's layout:
+        ({state_dict name: [_PackT]} of the forward's copies, {state_dict name: [_PackT]} of the data-gradient copies
+        of the convs in `dgrad`, keys of self._bwd).  The forward's weights are TF32-rounded fp32 with an fp16 twin in
+        fp16 engines (exact fp32 with conv_impl="simt"); the data gradient's are fp16."""
+        L, tf = _lib, self._fwd_transform
+        fw, dg = {}, {}
 
-    def _refresh_targets(self):
-        """{state_dict name: [_PackT]}: every derived copy of every trainable parameter, in the layouts the
-        constructor's host packing produces"""
-        L = _lib
-        self._pack_heads_backward()
-        tg = {}
-        bias = lambda name, dst: _PackT(name, dst, (1, 1, 1, dst.numel()), (0, 0, 0, 1), (0, 0, 0, 1), L.PACK_F32)
-        for key in self._bwd_src:       # trunk, FPN, RPN_Conv, RCNN_top.3, RCNN_kpts.0..10
-            if key == "rpn_heads":
+        def put(tg, name, *a, **k):
+            tg.setdefault(name, []).append(_PackT(name, *a, **k))
+
+        def flat(tg, name, dst, n, transform, **k):
+            put(tg, name, dst, (1, 1, 1, n), (0, 0, 0, 1), (0, 0, 0, 1), transform, **k)
+
+        # stem [64,3,7,7]: [64][7][7][3] fp32 (i1 = tap, i2 = co, i3 = ci); as 64 rows of the 147 taps in (ci, r, s)
+        # order, the GEMM's [64,160] over sb_stem_im2col's patches and the fused stem's fp16 [64,192]
+        name = "RCNN_layer0.0.weight"
+        put(fw, name, self.stem[0], (1, 49, 64, 3), (0, 1, 147, 49), (0, 3, 147, 1), L.PACK_F32)
+        sg = self.p["stem_gemm"]
+        put(fw, name, sg.w, (1, 1, 64, 147), (0, 0, 147, 1), (0, 0, 160, 1), tf, dst16=sg.w16)
+        put(fw, name, self.stem_w16, (1, 1, 64, 147), (0, 0, 147, 1), (0, 0, 192, 1), L.PACK_F16)
+        # trunk, FPN, RPN_Conv, RCNN_top.3, RCNN_kpts.0..10: forward [Cout][kh][kw][Cin] (i1 = tap, i2 = co,
+        # i3 = ci); data gradient [Cin][kh][kw][Cout], i1 = flipped tap t' (source tap T-1-t'), i2 = ci, i3 = co,
+        # the frozen-BN scale folded in for the trunk convs
+        for key, pc in self.p.items():
+            if key in ("stem_gemm", "rpn_heads", "RCNN_top.0"):
                 continue
-            tg[key + ".weight"] = self._conv_targets(key, key + ".weight")
-            if self.p[key].scale is None:
-                tg[key + ".bias"] = [bias(key + ".bias", self.p[key].shift)]
+            name, co, ci, T = key + ".weight", pc.Cout, pc.Cin, pc.kh * pc.kw
+            if T == 1:
+                flat(fw, name, pc.w, co * ci, tf, dst16=pc.w16)
+            else:
+                put(fw, name, pc.w, (1, T, co, ci), (0, 1, T * ci, T), (0, ci, T * ci, 1), tf, dst16=pc.w16)
+            if pc.scale is None:
+                flat(fw, key + ".bias", pc.shift, co, L.PACK_F32)
+            if key in dgrad:
+                put(dg, name, self._bwd[key].w16, (1, T, ci, co), (0, -1, T, ci * T), (0, co, T * co, 1),
+                    L.PACK_F16 if pc.scale is None else L.PACK_SCALE_F16, src_offset=T - 1, scale=pc.scale)
         # RPN heads: rows 0..5 / 6..23 of the fused head, columns 0..5 / 6..23 of its 64-column data-gradient copy
-        ph, bh = self.p["rpn_heads"], self._bwd["rpn_heads"]
+        ph = self.p["rpn_heads"]
         for key, r0, n in (("RCNN_rpn.RPN_cls_score", 0, 6), ("RCNN_rpn.RPN_bbox_pred_left_right", 6, 18)):
-            tg[key + ".weight"] = [
-                _PackT(key + ".weight", ph.w, (1, 1, 1, n * 1024), (0, 0, 0, 1), (0, 0, 0, 1), self._fwd_transform,
-                       dst_offset=r0 * 1024, dst16=ph.w16),
-                _PackT(key + ".weight", bh.w16, (1, 1, 1024, n), (0, 0, 1, 1024), (0, 0, 64, 1), L.PACK_F16,
-                       dst_offset=r0)]
-            tg[key + ".bias"] = [_PackT(key + ".bias", ph.shift, (1, 1, 1, n), (0, 0, 0, 1), (0, 0, 0, 1), L.PACK_F32,
-                                        dst_offset=r0)]
+            flat(fw, key + ".weight", ph.w, n * 1024, tf, dst_offset=r0 * 1024, dst16=ph.w16)
+            flat(fw, key + ".bias", ph.shift, n, L.PACK_F32, dst_offset=r0)
+            if "rpn_heads" in dgrad:
+                put(dg, key + ".weight", self._bwd["rpn_heads"].w16, (1, 1, 1024, n), (0, 0, 1, 1024), (0, 0, 64, 1),
+                    L.PACK_F16, dst_offset=r0)
         # RCNN_top.0 [2048,512,7,7]: forward [co][(ph, pw, c)], data gradient [(ph, pw, c)][co]
-        pt, bt = self.p["RCNN_top.0"], self._bwd["RCNN_top.0"]
-        tg["RCNN_top.0.weight"] = [
-            _PackT("RCNN_top.0.weight", pt.w, (1, 49, 2048, 512), (0, 1, 49 * 512, 49), (0, 512, 49 * 512, 1),
-                   self._fwd_transform, dst16=pt.w16),
-            _PackT("RCNN_top.0.weight", bt.w16, (1, 49, 512, 2048), (0, 1, 49, 49 * 512), (0, 512 * 2048, 2048, 1),
-                   L.PACK_F16)]
-        tg["RCNN_top.0.bias"] = [bias("RCNN_top.0.bias", pt.shift)]
+        pt = self.p["RCNN_top.0"]
+        put(fw, "RCNN_top.0.weight", pt.w, (1, 49, 2048, 512), (0, 1, 49 * 512, 49), (0, 512, 49 * 512, 1), tf,
+            dst16=pt.w16)
+        flat(fw, "RCNN_top.0.bias", pt.shift, 2048, L.PACK_F32)
+        if "RCNN_top.0" in dgrad:
+            put(dg, "RCNN_top.0.weight", self._bwd["RCNN_top.0"].w16, (1, 49, 512, 2048), (0, 1, 49, 49 * 512),
+                (0, 512 * 2048, 2048, 1), L.PACK_F16)
         # deconv [Cin,Cout,2,2]: phase (a, b) forward [co][ci] = W[ci, co, a, b]; data gradient [ci][(a, b, co)]
         name = "RCNN_kpts.12.weight"
-        tg[name] = [_PackT(name, self.deconv[a][b].w, (1, 256, 1, 256), (0, 4, 0, 1024), (0, 256, 0, 1),
-                           self._fwd_transform, src_offset=2 * a + b, dst16=self.deconv[a][b].w16)
-                    for a in range(2) for b in range(2)]
-        tg[name].append(_PackT(name, self._bwd["deconv"].w16, (1, 4, 256, 256), (0, 1, 1024, 4), (0, 256, 1024, 1),
-                               L.PACK_F16))
-        tg["RCNN_kpts.12.bias"] = [bias("RCNN_kpts.12.bias", self.deconv[a][b].shift) for a in range(2)
-                                   for b in range(2)]
+        for a in range(2):
+            for b in range(2):
+                pc = self.deconv[a][b]
+                put(fw, name, pc.w, (1, 256, 1, 256), (0, 4, 0, 1024), (0, 256, 0, 1), tf, src_offset=2 * a + b,
+                    dst16=pc.w16)
+                flat(fw, "RCNN_kpts.12.bias", pc.shift, 256, L.PACK_F32)
+        if "deconv" in dgrad:
+            put(dg, name, self._bwd["deconv"].w16, (1, 4, 256, 256), (0, 1, 1024, 4), (0, 256, 1024, 1), L.PACK_F16)
         # the fp32 linears and kpts_class: plain copies
-        for key, dst in zip(("RCNN_cls_score.weight", "RCNN_cls_score.bias", "RCNN_bbox_pred.weight",
-                             "RCNN_bbox_pred.bias", "RCNN_dim_orien_pred.weight", "RCNN_dim_orien_pred.bias",
-                             "kpts_class.weight", "kpts_class.bias"), self.fc + list(self.kpts_class)):
-            tg[key] = [bias(key, dst)]
-        return tg
+        for key, dst in zip(_FC + ("kpts_class.weight", "kpts_class.bias"), self.fc + list(self.kpts_class)):
+            flat(fw, key, dst, dst.numel(), L.PACK_F32)
+        return fw, dg
 
     @property
     def _fwd_transform(self):
         return _lib.PACK_F32 if self.exact else _lib.PACK_TF32
+
+    def _table(self, items, srcs):
+        """the planned host table of pack targets `items` reading srcs[name], and its device copy"""
+        L = _lib
+        for tp in items:
+            shape = (64, 3, 7, 7) if tp.name == "RCNN_layer0.0.weight" else self._trainable[tp.name]
+            assert srcs[tp.name].numel() == _numel(shape), tp.name
+        tab = (L.PackTarget * len(items))()
+        for i, tp in enumerate(items):
+            tp.fill(tab[i], srcs[tp.name])
+        n_tiles = ctypes.c_longlong()
+        L.check(L.load().sb_pack_plan(tab, len(items), ctypes.byref(n_tiles)), "sb_pack_plan")
+        return tab, torch.frombuffer(bytearray(memoryview(tab).cast("B")), dtype=torch.uint8).to(self.device)
+
+    def _pack_from_host(self, tg):
+        """pack the targets {name: [_PackT]} in one launch from the host masters, uploaded for it and then dropped"""
+        L = _lib
+        with torch.cuda.device(self.device):
+            srcs = {n: self._masters[n].to(self.device) for n in tg}
+            tab, dev = self._table([tp for ts in tg.values() for tp in ts], srcs)
+            L.check(L.load().sb_pack_weights(tab, ops.ptr(dev), len(tab), L.stream_ptr()), "sb_pack_weights")
 
     def refresh_weights(self, params):
         """Rewrite, in place and on the device, every copy this engine holds of the parameters in `params`
         ({state_dict name: fp32 contiguous device tensor in the reference's layout}, any subset of the trainable
         names): the forward's packed weights (TF32-rounded fp32 and fp16), the data gradient's transposed fp16
         copies (taps flipped, frozen-BN scale folded in), the fused RPN head and its data-gradient copy, the
-        (ph, pw, c)-ordered RCNN_top.0, the four deconv phases, biases, the linears and kpts_class.  The result is
-        bit-identical to what the constructor packs on the host from the same values.  No tensor is reallocated, so
-        CUDA graphs captured over the forward or backward stay valid.  Frozen tensors (the stem, frozen layers, the
-        BN scale and shift) are never written.
+        (ph, pw, c)-ordered RCNN_top.0, the four deconv phases, biases, the linears and kpts_class.  The targets are
+        the ones the constructor and the first backward pack from, so the result is bit-identical to a new engine
+        built from the same values.  No tensor is reallocated, so CUDA graphs captured over the forward or backward
+        stay valid.  Frozen tensors (the stem, frozen layers, the BN scale and shift) are never written.
         One launch (sb_pack_weights).  The table of a new set of (name, tensor) pairs is built and uploaded on first
         use: make that first call outside any graph capture; later calls with the same tensors are
         graph-capturable and do not synchronise."""
         L = _lib
         if not hasattr(self, "_refresh_cache"):
             self._refresh_cache = {}
-            self._refresh_tg = self._refresh_targets()
+            # the data-gradient copies first: packed later from the host masters, they would miss this refresh
+            self._pack_heads_backward()
+            fw, dg = self._pack_targets(self._bwd)
+            self._refresh_tg = {n: fw[n] + dg.get(n, []) for n in self._trainable}
         for n, t in params.items():
             if n not in self._refresh_tg:
                 raise KeyError("not a trainable parameter of this engine: %s" % n)
@@ -920,25 +930,10 @@ class StereoRCNNEngine(object):
         key = tuple(sorted((n, t.data_ptr()) for n, t in params.items()))
         ent = self._refresh_cache.get(key)
         if ent is None:
-            items = [tp for n in sorted(params) for tp in self._refresh_tg[n]]
-            for tp in items:
-                assert params[tp.name].numel() == _numel(self._refresh_shape(tp.name)), tp.name
-            tab = (L.PackTarget * len(items))()
-            for i, tp in enumerate(items):
-                tp.fill(tab[i], params[tp.name])
-            n_tiles = ctypes.c_longlong()
-            L.check(L.load().sb_pack_plan(tab, len(items), ctypes.byref(n_tiles)), "sb_pack_plan")
-            raw = bytes(memoryview(tab).cast("B"))
-            dev = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(self.device)
-            ent = self._refresh_cache[key] = (tab, dev, len(items), [params[n] for n in sorted(params)])
-        tab, dev, n, _keep = ent
-        L.check(L.load().sb_pack_weights(tab, ops.ptr(dev), n, L.stream_ptr()), "sb_pack_weights")
-
-    def _refresh_shape(self, name):
-        if not hasattr(self, "_trainable_shapes"):
-            self._trainable_shapes = dict(trainable_trunk_fpn_params(0) + trainable_rpn_params() +
-                                          trainable_rcnn_head_params(self.n_classes))
-        return self._trainable_shapes[name]
+            tab, dev = self._table([tp for n in sorted(params) for tp in self._refresh_tg[n]], params)
+            ent = self._refresh_cache[key] = (tab, dev, [params[n] for n in sorted(params)])
+        tab, dev, _keep = ent
+        L.check(L.load().sb_pack_weights(tab, ops.ptr(dev), len(tab), L.stream_ptr()), "sb_pack_weights")
 
     @torch.no_grad()
     def forward(self, im_left, im_right, im_info, cfg_key="TEST", keep_features=False, im_h=None,

@@ -622,17 +622,10 @@ def stem_im2col(im_nchw):
     return out
 
 
-def pack_stem_w16(weight):
-    """[64,3,7,7] stem weights -> fp16 [64,192] in sb_stem_conv_tc's K layout: tap (ci, r, s) at
-    k = ci*49 + r*7 + s, zero padded from 147 to three 64-wide K-steps"""
-    w = torch.zeros(64, 192, dtype=torch.float32)
-    w[:, :147] = weight.detach().float().cpu().reshape(64, 147)
-    return w.to(torch.float16)
-
-
 def stem_conv_tc(im_nchw, w16, scale, shift):
     """stem conv7x7/2 + frozen BN + ReLU as an implicit tensor-core GEMM (patch gather inside the kernel)
-    -> fp16 NHWC [N, Ho, Wo, 64]; w16: fp16 [64,192] from pack_stem_w16"""
+    -> fp16 NHWC [N, Ho, Wo, 64]; w16: fp16 [64,192], tap (ci, r, s) of output channel co at [co][ci*49 + r*7 + s],
+    zero padded from 147 to three 64-wide K-steps (the engine's stem_w16)"""
     L = _l.load()
     N, _, H, W = im_nchw.shape
     Ho, Wo = (H + 6 - 7) // 2 + 1, (W + 6 - 7) // 2 + 1

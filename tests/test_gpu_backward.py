@@ -131,15 +131,16 @@ SENT32 = 0x7FA5A5A5                  # NaN bit pattern: bytes the data gradient 
 
 @pytest.mark.parametrize("case", DGRAD_CASES)
 @pytest.mark.parametrize("epi", ["plain", "mask_residual"])
-def test_dgrad_exact(case, epi):
+def test_dgrad_exact_on_restated_weights(case, epi):
     N, H, W, Cin, Cout, k, stride = case
     g = torch.Generator().manual_seed(2)
     Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
     w = torch.randn(Cout, Cin, k, k, generator=g) / (Cin * k * k) ** 0.5
     s = torch.rand(Cout, generator=g) + 0.5
     dy = torch.randn(N, Ho, Wo, Cout, generator=g)
-    pc = E._DgradConv(w, s, k // 2, "cuda")
-    ws = pc.w16.float().cpu().permute(3, 0, 1, 2).flip(2, 3)           # the fp16-rounded s * w actually used
+    # the data gradient's weights, as the engine packs them: [Cin][kh][kw][Cout] fp16, taps flipped, scale folded in
+    w16 = (w * s.view(-1, 1, 1, 1)).flip(2, 3).permute(1, 2, 3, 0).contiguous().half()
+    ws = w16.float().permute(3, 0, 1, 2).flip(2, 3)                     # the fp16-rounded s * w actually used
     ref = F.conv_transpose2d(nchw(h16(dy)).double(), ws.double(), stride=stride, padding=k // 2,
                              output_padding=(H - 1 - (Ho - 1) * stride))
     ref = ref.permute(0, 2, 3, 1)
@@ -159,7 +160,7 @@ def test_dgrad_exact(case, epi):
             full[:, ::stride, ::stride] = res_cpu.double()
             ref = ref + full
         ref = torch.where(mask_cpu.float() > 0, ref, torch.zeros_like(ref))
-    d = G.conv_desc(dy.half().cuda(), pc.w16, out, pc.Cin, pc.Cout, k, k, 1, k // 2, Ho, Wo, residual=res,
+    d = G.conv_desc(dy.half().cuda(), w16.cuda(), out, Cout, Cin, k, k, 1, k // 2, Ho, Wo, residual=res,
                     out_strides=(H * W * Cin, stride * W * Cin, stride * Cin))
     G.conv2d_dgrad(d, mask)
     torch.cuda.synchronize()

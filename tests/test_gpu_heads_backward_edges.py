@@ -331,9 +331,14 @@ def test_flag_kpts_reduce_overflow_only():
 
 # ================================================================================================ the chain ====
 @pytest.fixture(scope="module")
-def chain():
+def sd():
+    return OM.make_state_dict(3)
+
+
+@pytest.fixture(scope="module")
+def chain(sd):
     H, W = _small_hw()
-    eng = EN.StereoRCNNEngine(OM.make_state_dict(3), "cuda", precision="fp16")
+    eng = EN.StereoRCNNEngine(sd, "cuda", precision="fp16")
     with torch.no_grad():
         feats = {B: eng.trunk_fpn(_pairs(H, W, B, 5).cuda()) for B in (1, 2)}
     return eng, feats, H, W
@@ -360,7 +365,7 @@ WGRAD_TOL = 1e-4
 
 
 @pytest.mark.parametrize("B,R,dropout", [(2, 1024, False), (2, 1024, True), (1, 1, False), (2, 129, True)])
-def test_heads_backward_vs_float64(chain, B, R, dropout):
+def test_heads_backward_vs_float64_from_state_dict(chain, sd, B, R, dropout):
     eng, _, H, W = chain
     rl, rr = cuda(*E.synth_rois(R, B, H, W))
     words = _words((2, R, 2048), 40 + R) if dropout else None
@@ -372,7 +377,7 @@ def test_heads_backward_vs_float64(chain, B, R, dropout):
     torch.cuda.synchronize()
     assert int(eng.found_inf.item()) == 0
     with torch.no_grad():
-        ref, rpool, mid = _heads_backward_ref(eng, saved, d, gs)
+        ref, rpool, mid = _heads_backward_ref(eng, sd, saved, d, gs)
     errs = {n: l2_err(got[n], ref[n]) for n in ref}
     errs.update({"d" + k: l2_err(dpool[k], rpool[k]) for k in rpool})
     errs.update({k: l2_err(a, b) for k, (a, b) in mid.items()})

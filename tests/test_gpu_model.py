@@ -220,7 +220,7 @@ def test_stem_maxpool_subsample():
 
 
 @pytest.mark.parametrize("shape", [(2, 67, 102), (1, 40, 77), (3, 7, 8), (1, 130, 260)])
-def test_stem_conv_tc_fused_gather(shape):
+def test_stem_conv_tc_fused_gather_restated_weights(shape):
     """the stem as an implicit tensor-core GEMM (patches gathered inside the kernel, no patch matrix): against the
     convolution (resnet.py:111-113) of the SAME fp16-rounded image and weights in fp64 -- what the tensor core computes
     up to fp32 accumulation order and the fp16 rounding of the result -- on even widths (8-byte loads), odd widths
@@ -231,7 +231,9 @@ def test_stem_conv_tc_fused_gather(shape):
     im = torch.randn(N, 3, H, W, generator=g) * 50
     s = sd["RCNN_layer0.1.weight"] / torch.sqrt(sd["RCNN_layer0.1.running_var"] + 1e-5)
     b = sd["RCNN_layer0.1.bias"] - sd["RCNN_layer0.1.running_mean"] * s
-    w16 = G.pack_stem_w16(sd["RCNN_layer0.0.weight"])
+    w16 = torch.zeros(64, 192)                  # sb_stem_conv_tc's K layout: tap (ci, r, s) at ci*49 + r*7 + s
+    w16[:, :147] = sd["RCNN_layer0.0.weight"].reshape(64, 147)
+    w16 = w16.half()
     y = G.stem_conv_tc(cu(im), cu(w16), cu(s), cu(b))
     assert y.shape == (N, (H - 1) // 2 + 1, (W - 1) // 2 + 1, 64) and y.dtype == torch.float16
     conv = F.conv2d(im.half().double(), sd["RCNN_layer0.0.weight"].half().double(), stride=2, padding=3)

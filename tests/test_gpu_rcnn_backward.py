@@ -299,12 +299,11 @@ def test_new_entry_points_reject_invalid_arguments():
 
 
 # ---------------------------------------------------------------- 4. heads_backward layer by layer against float64
-def _heads_backward_ref(eng, saved, d, gs):
+def _heads_backward_ref(eng, sd, saved, d, gs):
     """float64 on the GPU, layer by layer: fp16-rounded weights, the engine's saved fp16 operands and masks, and the
     engine's own fp16 inter-layer gradients (recomputed with the same deterministic kernels, so the same bits as inside
     heads_backward) as each layer's input.  Returns the references and the engine's inter-layer fp32 gradients with
     theirs."""
-    src = eng._bwd_src
     R = saved.R
     d_cls, d_box, d_dim, dkp, dl, dr = d
     keep = 1.25 if saved.dropout else 1.0
@@ -326,7 +325,7 @@ def _heads_backward_ref(eng, saved, d, gs):
     x0 = saved.top0.view(R, 2048).double()
     ref["RCNN_top.3.weight"] = (dz16.double().t() @ x0 / gs).view(2048, 2048, 1, 1)
     ref["RCNN_top.3.bias"] = dz32.double().sum(0) / gs
-    w3 = h16(src["RCNN_top.3"][0].view(2048, 2048).cuda())
+    w3 = h16(sd["RCNN_top.3.weight"].view(2048, 2048).cuda())
     t3 = eng._bwd["RCNN_top.3"]
     d0_32 = torch.empty(R, 1, 1, 2048, device="cuda")
     d0_16 = torch.empty(R, 1, 1, 2048, dtype=torch.float16, device="cuda")
@@ -338,7 +337,7 @@ def _heads_backward_ref(eng, saved, d, gs):
     pooled = saved.pooled_box.view(R, -1).double()
     ref["RCNN_top.0.weight"] = (d0.t() @ pooled / gs).view(2048, 7, 7, 512).permute(0, 3, 1, 2)
     ref["RCNN_top.0.bias"] = d0_32.double().sum((0, 1, 2)) / gs
-    w0 = h16(E._pack_conv(eng._heads_bwd_src["RCNN_top.0"]).reshape(2048, -1).cuda())
+    w0 = h16(sd["RCNN_top.0.weight"].permute(0, 2, 3, 1).reshape(2048, -1).cuda())     # [co][(ph, pw, c)]
     dpool = (d0 @ w0 / gs).view(R, 7, 7, 512)
     ph, dw, db, dbu = _kpts_ref(saved.up, eng.kpts_class[0], dkp, dl, dr, gs)
     ref["kpts_class.weight"], ref["kpts_class.bias"], ref["RCNN_kpts.12.bias"] = dw.view(6, 256, 1, 1), db, dbu
@@ -348,7 +347,7 @@ def _heads_backward_ref(eng, saved, d, gs):
     x6 = saved.kpts[5].double()
     dph = dup16.double()                                                # [R,14,14,(a,b,co)]
     ref["RCNN_kpts.12.weight"] = torch.einsum("rijp,rijc->pc", dph, x6).view(2, 2, 256, 256).permute(3, 2, 0, 1) / gs
-    wd = h16(eng._heads_bwd_src["deconv"].cuda())                       # [ci,co,a,b]
+    wd = h16(sd["RCNN_kpts.12.weight"].cuda())                          # [ci,co,a,b]
     wf = wd.permute(2, 3, 1, 0).reshape(1024, 256)
     g32, g16 = eng._dgrad(dup16, "deconv", mask=saved.kpts[5])
     mid["d kpts.10 out"] = (g32, (dph @ wf) * (x6 > 0).double())
@@ -359,7 +358,7 @@ def _heads_backward_ref(eng, saved, d, gs):
         ref[key + ".weight"] = torch.nn.grad.conv2d_weight(xin.permute(0, 3, 1, 2), (256, 256, 3, 3), g,
                                                            padding=1) / gs
         ref[key + ".bias"] = g32.double().sum((0, 1, 2)) / gs
-        nxt = F.conv_transpose2d(g, h16(src[key][0].cuda()), padding=1).permute(0, 2, 3, 1)
+        nxt = F.conv_transpose2d(g, h16(sd[key + ".weight"].cuda()), padding=1).permute(0, 2, 3, 1)
         if i > 0:
             g32, g16 = eng._dgrad(g16, key, mask=saved.kpts[i - 1])
             mid["d kpts.%d out" % (2 * i - 2)] = (g32, nxt * (xin > 0).double())
@@ -367,7 +366,7 @@ def _heads_backward_ref(eng, saved, d, gs):
 
 
 @pytest.mark.parametrize("dropout", [False, True])
-def test_heads_backward_vs_float64(sd, dropout):
+def test_heads_backward_vs_float64_from_state_dict(sd, dropout):
     H, W = _small_hw()
     eng = E.StereoRCNNEngine(sd, "cuda", precision="fp16")
     feats, rl, rr = _test_rois(eng, H, W, 1)
@@ -384,7 +383,7 @@ def test_heads_backward_vs_float64(sd, dropout):
     assert int(eng.found_inf.item()) == 0
     assert sorted(got) == sorted(n for n, _ in E.trainable_rcnn_head_params())
     with torch.no_grad():
-        ref, rpool, mid = _heads_backward_ref(eng, saved, d, gs)
+        ref, rpool, mid = _heads_backward_ref(eng, sd, saved, d, gs)
     errs = {n: l2_err(got[n], ref[n]) for n in ref}
     errs.update({"d" + k: l2_err(dpool[k], rpool[k]) for k in rpool})
     errs.update({k: l2_err(a, b) for k, (a, b) in mid.items()})

@@ -231,12 +231,13 @@ def test_wgrad_acc_rejects_invalid_arguments():
 
 
 # ---------------------------------------------------------------- 4. rpn_backward alone against float64
-def _rpn_backward_ref(eng, saved, d_cls, d_box):
+def _rpn_backward_ref(sd, saved, d_cls, d_box):
     """float64: heads and RPN_Conv on the engine's fp16 operands (fp16-rounded weights, saved cat, fp16 P levels), the
     ReLU replaced by the saved mask cat > 0; d cat rounded to fp16 where the kernels read it as an fp16 operand"""
     B, offs = saved.B, saved.offs
-    wh = eng._bwd_src["rpn_heads"][0][:24, :, 0, 0].half().double()          # [24,1024]
-    wc = eng._bwd_src["RCNN_rpn.RPN_Conv"][0].half().double()                # [512,256,3,3]
+    wh = torch.cat([sd["RCNN_rpn.RPN_cls_score.weight"], sd["RCNN_rpn.RPN_bbox_pred_left_right.weight"]])
+    wh = wh[:, :, 0, 0].half().double()                                       # [24,1024]
+    wc = sd["RCNN_rpn.RPN_Conv.weight"].half().double()                      # [512,256,3,3]
     P = offs[-1]
     dx = torch.zeros(B, P, 24, dtype=torch.float64)       # exact: the bias gradients read the fp32 twin
     dx[:, :, 0:6] = d_cls.cpu().double().view(B, P, 6)
@@ -270,7 +271,7 @@ def _rpn_backward_ref(eng, saved, d_cls, d_box):
 
 
 @pytest.mark.parametrize("B", [1, 2])
-def test_rpn_backward_vs_float64(sd, B):
+def test_rpn_backward_vs_float64_from_state_dict(sd, B):
     H, W = _small_hw()
     eng = E.StereoRCNNEngine(sd, "cuda", precision="fp16")
     with torch.no_grad():
@@ -284,7 +285,7 @@ def test_rpn_backward_vs_float64(sd, B):
     torch.cuda.synchronize()
     assert int(eng.found_inf.item()) == 0
     assert sorted(got) == sorted(n for n, _ in E.trainable_rpn_params())
-    ref, rdp = _rpn_backward_ref(eng, saved, d_cls, d_box)
+    ref, rdp = _rpn_backward_ref(sd, saved, d_cls, d_box)
     errs = {n: l2_err(got[n], ref[n]) for n in ref}
     errs.update({"d" + k: l2_err(dps[k], rdp[k]) for k in LEVELS})
     print("rpn_backward B=%d vs float64: %s" % (B, ", ".join("%s %.2e" % kv for kv in sorted(errs.items()))))
