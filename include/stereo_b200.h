@@ -587,6 +587,10 @@ int sb_pack_weights(const sb_pack_target* targets, const sb_pack_target* targets
  *   out_right are sb_prep_image of left / right.  *flip != 0 (minibatch.py:116-119): out_left is sb_prep_image of the
  *   column-mirrored RIGHT frame and out_right of the column-mirrored LEFT frame, bit for bit, without materialising
  *   the mirrored frames.
+ * sb_prep_stereo_pairs -- sb_prep_stereo_pair for B pairs of one frame shape in one launch (the same kernel; the
+ *   single-pair entry point is its B = 1 launch): left / right uint8 [B,H,W,3], flip int32 [B] on the DEVICE (one
+ *   flag per pair, so one captured launch serves any mix of flipped and unflipped pairs), out_left / out_right fp32
+ *   [B,3,Ho,Wo].  Pair b is sb_prep_stereo_pair of frames b with flag flip[b], bit for bit.  1 <= B <= 32767.
  * sb_train_gt -- the ground truth of a step (minibatch.py:43-85, roibatchLoader.py:72-107) for B images, one CTA per
  *   image.  Inputs are the roidb rows of each image at a fixed capacity N <= 1024: boxes_left / boxes_right /
  *   boxes_merge [B,N,4], gt_classes [B,N] int32, dim_orien [B,N,4] (w, h, l, alpha), kpts [B,N,6], n_rows [B] int32
@@ -602,9 +606,12 @@ int sb_pack_weights(const sb_pack_target* targets, const sb_pack_target* targets
  *   and counter (i / 4, stream_id, *step lo, *step hi); *step is a uint64 on the DEVICE.  The words do not depend on
  *   the launch geometry.  Replaces the torch.randint refills of train.random_words between the replays of a step.
  * sb_step_advance -- *step += 1 in one thread: the last node of a captured step, so every replay draws new words.
- * SB_EINVAL before any launch for a null pointer, a non-positive size or scale, N > 1024 or n == 0.            */
+ * SB_EINVAL before any launch for a null pointer, a non-positive size or scale, B outside its range, N > 1024 or
+ * n == 0.                                                                                                         */
 int sb_prep_stereo_pair(const uint8_t* left, const uint8_t* right, int H, int W, double scale, int rgb_input,
                         const int* flip, float* out_left, float* out_right, sb_stream_t stream);
+int sb_prep_stereo_pairs(const uint8_t* left, const uint8_t* right, int B, int H, int W, double scale, int rgb_input,
+                         const int* flip, float* out_left, float* out_right, sb_stream_t stream);
 int sb_train_gt(const float* boxes_left, const float* boxes_right, const float* boxes_merge, const int* gt_classes,
                 const float* dim_orien, const float* kpts, const int* n_rows, const unsigned* words, int B, int N,
                 float im_scale, int im_width, float* gt_left, float* gt_right, float* gt_merge,

@@ -11,17 +11,20 @@ namespace {
 
 constexpr int kMaxGtRows = 1024;       // annotation-row capacity N of sb_train_gt (one CTA ranks them in shared memory)
 constexpr int kMaxNumGt = 30;          // cfg.MAX_NUM_GT_BOXES (config.py:283)
+constexpr int kMaxPrepPairs = 32767;   // 2 B CTAs along grid z, whose limit is 65535
 
+// blockIdx.z = 2 b + side: pair b of the batch, side 0 (left blob) or 1 (right blob)
 __global__ void __launch_bounds__(256)
 prep_stereo_pair_kernel(const uint8_t* __restrict__ left, const uint8_t* __restrict__ right, int H, int W, double inv,
                         int rgb, const int* __restrict__ flip, float* __restrict__ out_left,
                         float* __restrict__ out_right, int Ho, int Wo) {
-    const int x = blockIdx.x * 256 + threadIdx.x, y = blockIdx.y;
+    const int x = blockIdx.x * 256 + threadIdx.x, y = blockIdx.y, b = blockIdx.z >> 1, side = blockIdx.z & 1;
     if (x >= Wo) return;
-    const int f = *flip != 0;
+    const int f = flip[b] != 0;
+    const size_t in_off = (size_t)b * H * W * 3, out_off = (size_t)b * 3 * Ho * Wo;
     // flipped: the left blob is the mirrored right frame and the right blob the mirrored left frame
-    const uint8_t* src = (blockIdx.z == 0) != (f != 0) ? left : right;
-    prep_pixel(src, H, W, inv, rgb, f, blockIdx.z == 0 ? out_left : out_right, Ho, Wo, x, y);
+    const uint8_t* src = ((side == 0) != (f != 0) ? left : right) + in_off;
+    prep_pixel(src, H, W, inv, rgb, f, (side == 0 ? out_left : out_right) + out_off, Ho, Wo, x, y);
 }
 
 __global__ void __launch_bounds__(256)
@@ -119,18 +122,24 @@ __global__ void step_advance_kernel(unsigned long long* step) { *step += 1ULL; }
 
 }  // namespace
 
-extern "C" int sb_prep_stereo_pair(const uint8_t* left, const uint8_t* right, int H, int W, double scale,
-                                   int rgb_input, const int* flip, float* out_left, float* out_right,
-                                   sb_stream_t stream) {
+extern "C" int sb_prep_stereo_pairs(const uint8_t* left, const uint8_t* right, int B, int H, int W, double scale,
+                                    int rgb_input, const int* flip, float* out_left, float* out_right,
+                                    sb_stream_t stream) {
     int Ho = 0, Wo = 0;
-    if (!left || !right || !flip || !out_left || !out_right || sb_prep_image_size(H, W, scale, &Ho, &Wo) != SB_OK ||
-        Ho < 1 || Wo < 1)
+    if (!left || !right || !flip || !out_left || !out_right || B < 1 || B > kMaxPrepPairs ||
+        sb_prep_image_size(H, W, scale, &Ho, &Wo) != SB_OK || Ho < 1 || Wo < 1)
         return SB_EINVAL;
-    prep_stereo_pair_kernel<<<dim3(sb_div_up(Wo, 256), Ho, 2), 256, 0, sb_cs(stream)>>>(
+    prep_stereo_pair_kernel<<<dim3(sb_div_up(Wo, 256), Ho, 2 * B), 256, 0, sb_cs(stream)>>>(
         left, right, H, W, 1.0 / scale, rgb_input, flip, out_left, out_right, Ho, Wo);
     SB_LAUNCHED();
     SB_CHECK_LAUNCH();
     return SB_OK;
+}
+
+extern "C" int sb_prep_stereo_pair(const uint8_t* left, const uint8_t* right, int H, int W, double scale,
+                                   int rgb_input, const int* flip, float* out_left, float* out_right,
+                                   sb_stream_t stream) {
+    return sb_prep_stereo_pairs(left, right, 1, H, W, scale, rgb_input, flip, out_left, out_right, stream);
 }
 
 extern "C" int sb_train_gt(const float* boxes_left, const float* boxes_right, const float* boxes_merge,

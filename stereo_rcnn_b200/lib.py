@@ -176,6 +176,8 @@ _SIGS = {
     # the training side of the input pipeline
     "sb_prep_stereo_pair": (c_int, [c_void_p, c_void_p, c_int, c_int, c_double, c_int, c_void_p, c_void_p, c_void_p,
                                     c_void_p]),
+    "sb_prep_stereo_pairs": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_int, c_void_p, c_void_p,
+                                     c_void_p, c_void_p]),
     "sb_train_gt": (c_int, [c_void_p] * 8 + [c_int, c_int, c_float, c_int] + [c_void_p] * 6 + [c_void_p]),
     "sb_random_words": (c_int, [ctypes.c_ulonglong, c_void_p, ctypes.c_uint, c_void_p, c_size_t, c_void_p]),
     "sb_step_advance": (c_int, [c_void_p, c_void_p]),

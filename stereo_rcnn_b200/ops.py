@@ -848,20 +848,25 @@ def prep_image_size(H, W, scale):
 
 
 def prep_stereo_pair(left_u8, right_u8, scale, flip, rgb_input=False, out=None):
-    """_get_image_blob (minibatch.py:89-131) for one pair in one launch: two uint8 [H,W,3] frames -> two fp32
-    [3,Ho,Wo] blobs.  flip: int32 [1] device tensor; when set the left blob is prep_image of the column-mirrored
-    right frame and the right blob of the mirrored left frame (minibatch.py:116-119).  out: (left, right) to write"""
+    """_get_image_blob (minibatch.py:89-131) for one pair or a batch of pairs in one launch: uint8 frames [H,W,3]
+    (one pair, flip int32 [1], blobs fp32 [3,Ho,Wo]) or [B,H,W,3] (B pairs, flip int32 [B], blobs [B,3,Ho,Wo]).
+    flip: device tensor; where set the left blob of the pair is prep_image of the column-mirrored right frame and the
+    right blob of the mirrored left frame (minibatch.py:116-119).  out: (left, right) to write"""
     L = _l.load()
-    assert left_u8.dtype == torch.uint8 and left_u8.dim() == 3 and left_u8.shape[2] == 3
+    assert left_u8.dtype == torch.uint8 and left_u8.dim() in (3, 4) and left_u8.shape[-1] == 3
     assert right_u8.dtype == torch.uint8 and right_u8.shape == left_u8.shape and flip.dtype == torch.int32
-    H, W = left_u8.shape[:2]
+    lead = tuple(left_u8.shape[:-3])
+    B = lead[0] if lead else 1
+    assert flip.numel() == B
+    H, W = left_u8.shape[-3:-1]
     ho, wo = ctypes.c_int(), ctypes.c_int()
     check(L.sb_prep_image_size(H, W, float(scale), ctypes.byref(ho), ctypes.byref(wo)), "sb_prep_image_size")
+    shape = lead + (3, ho.value, wo.value)
     if out is None:
-        out = tuple(torch.empty(3, ho.value, wo.value, dtype=torch.float32, device=left_u8.device) for _ in range(2))
-    assert all(tuple(o.shape) == (3, ho.value, wo.value) and o.dtype == torch.float32 for o in out)
-    check(L.sb_prep_stereo_pair(ptr(left_u8), ptr(right_u8), H, W, float(scale), 1 if rgb_input else 0, ptr(flip),
-                                ptr(out[0]), ptr(out[1]), stream_ptr()), "sb_prep_stereo_pair")
+        out = tuple(torch.empty(shape, dtype=torch.float32, device=left_u8.device) for _ in range(2))
+    assert all(tuple(o.shape) == shape and o.dtype == torch.float32 for o in out)
+    check(L.sb_prep_stereo_pairs(ptr(left_u8), ptr(right_u8), B, H, W, float(scale), 1 if rgb_input else 0, ptr(flip),
+                                 ptr(out[0]), ptr(out[1]), stream_ptr()), "sb_prep_stereo_pairs")
     return out
 
 

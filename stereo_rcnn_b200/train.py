@@ -459,12 +459,13 @@ class Trainer(object):
     overflow) writes no master, momentum or packed weight and counts itself in `skipped`: GradScaler's skip, the one
     deliberate difference from the reference.  The defaults are the reference's (config.py:22-46,
     trainval_net.py:153-168,226).  `engine` must have been built from `state_dict` (fp16 operands); the constructor
-    uploads the refresh table and synchronises once."""
+    uploads the refresh table and synchronises once.  At world > 1 `rank` is dist.get_rank(), otherwise 0."""
 
     def __init__(self, engine, state_dict, fixed_blocks=1, lr=1e-3, momentum=0.9, weight_decay=1e-4,
                  double_bias=False, bias_decay=False, clip_norm=10.0, grad_scale=1.0, world=1, dist=None, seed=0):
         self.engine, self.fixed_blocks, self.momentum = engine, int(fixed_blocks), float(momentum)
         self.clip_norm, self.grad_scale, self.world, self.dist = float(clip_norm), float(grad_scale), int(world), dist
+        self.rank = int(dist.get_rank()) if self.world > 1 and dist is not None else 0
         dev = engine.device
         named = trainable_names(fixed_blocks, engine.n_classes)
         self.names = [n for n, _ in named]
@@ -520,20 +521,23 @@ class Trainer(object):
         return losses, self.total, self.norm, self.skipped
 
     def step_from_frames(self, inp):
-        """One training step from the buffers of a StepInputs (one stereo pair): sb_prep_stereo_pair, the random words
-        of this step (sb_random_words keyed by `seed` and the device step counter, one stream id per tensor),
-        sb_train_gt, step, then sb_step_advance -- so the next call, or the next replay of a captured call, draws new
-        words; a skipped (overflowed) step advances too.  Returns what step returns.  Outside a stream capture the
-        current stream first waits for inp.load's copies and afterwards marks the buffers as consumed; a captured call
-        holds the kernels only, and whoever replays it calls inp.ready() before and inp.release() after."""
+        """One training step from the buffers of a StepInputs (its B stereo pairs): sb_prep_stereo_pairs, the random
+        words of this step (sb_random_words keyed by `seed` and the device step counter; tensor i of
+        inp.word_tensors takes stream id 5 rank + i, so every rank draws its own words and rank 0 those of a
+        one-process run), sb_train_gt, step, then sb_step_advance -- so the next call, or the next replay of a captured
+        call, draws new words; a skipped (overflowed) step advances too.  Returns what step returns.  Outside a stream
+        capture the current stream first waits for inp.load's copies and afterwards marks the buffers as consumed; a
+        captured call holds the kernels only, and whoever replays it calls inp.ready() before and inp.release()
+        after."""
         capturing = torch.cuda.is_current_stream_capturing()
         if not capturing:
             inp.ready()
         from .ops import prep_stereo_pair
         prep_stereo_pair(inp.left_u8, inp.right_u8, inp.scale, inp.flip, rgb_input=inp.rgb_input,
-                         out=(inp.im_left[0], inp.im_right[0]))
+                         out=(inp.im_left, inp.im_right))
+        n_ids = len(inp.word_tensors)
         for stream_id, t in enumerate(inp.word_tensors):
-            fill_random_words(t, self.seed, self.step_count, stream_id)
+            fill_random_words(t, self.seed, self.step_count, n_ids * self.rank + stream_id)
         train_gt(inp.rows, inp.n_rows, inp.shuffle_words, inp.scale, inp.im_left.shape[3], out=inp.gt)
         out = self.step(inp.im_left, inp.im_right, *inp.gt[:5], inp.keys, inp.words, inp.rpn_keys,
                         dropout_words=inp.dropout_words)
@@ -580,29 +584,43 @@ class Trainer(object):
 
 
 class StepInputs(object):
-    """The static buffers of one in-flight step_from_frames at one frame shape: the uint8 frame pair, the roidb rows
-    at capacity `max_rows` with their count, the flip flag, the two blobs, the ground truth of the step and its random
-    words.  load() fills the inputs from pinned host memory on a copy stream of its own, so with two StepInputs the
-    copy of entry k + 1 overlaps step k.  frame_hw: (H, W) of the camera frames; scale: im_scale of the blob
-    (target size / shorter side, blob.py:51); rgb_input: the frames are RGB, as image decoders give them
+    """The static buffers of one in-flight step_from_frames over `batch` stereo pairs of one frame shape: the uint8
+    frame pairs [B,H,W,3], the roidb rows [B,N,.] at capacity N = `max_rows` with their counts n_rows [B], the flip
+    flags [B], the blobs [B,3,Ho,Wo], the ground truth of the step ([B,30,.], num_boxes [B]) and its random words in
+    the shapes loss_gradients documents (keys [B,R+K], words [B,S], rpn_keys [B,A], the shuffle words [B,N], dropout
+    words [2,B*S,2048]).  load() fills the inputs from pinned host memory on a copy stream of its own, so with two
+    StepInputs the copy of batch k + 1 overlaps step k.  frame_hw: (H, W) of the camera frames; scale: im_scale of the
+    blob (target size / shorter side, blob.py:51); rgb_input: the frames are RGB, as image decoders give them
     (minibatch.py:111-114), not BGR."""
 
-    def __init__(self, frame_hw, scale, device, max_rows=64, rgb_input=True, rois_per_image=None, post_nms_top_n=None):
+    def __init__(self, frame_hw, scale, device, batch=1, max_rows=64, rgb_input=True, rois_per_image=None,
+                 post_nms_top_n=None):
         from .ops import CFG as OPS_CFG
         L = _l.load()
-        H, W = int(frame_hw[0]), int(frame_hw[1])
+        H, W, B = int(frame_hw[0]), int(frame_hw[1]), int(batch)
+        if B < 1:
+            raise ValueError("a StepInputs holds at least one pair, not %d" % B)
         self.frame_hw, self.scale, self.rgb_input, self.device, N = (H, W), float(scale), bool(rgb_input), device, int(max_rows)
+        self.batch = B
         ho, wo = ctypes.c_int(), ctypes.c_int()
         check(L.sb_prep_image_size(H, W, self.scale, ctypes.byref(ho), ctypes.byref(wo)), "sb_prep_image_size")
         Ho, Wo = ho.value, wo.value
         S = int(rois_per_image or CFG["BATCH_SIZE"])
         R = int(post_nms_top_n or OPS_CFG["TRAIN"]["RPN_POST_NMS_TOP_N"])
-        A = len(OPS_CFG["ANCHOR_RATIOS"]) * sum((-(-Ho // s)) * (-(-Wo // s)) for s in OPS_CFG["FPN_FEAT_STRIDES"])
-        host = {"left_u8": torch.empty(H, W, 3, dtype=torch.uint8), "right_u8": torch.empty(H, W, 3, dtype=torch.uint8),
-                "gt_classes": torch.zeros(1, N, dtype=torch.int32), "n_rows": torch.zeros(1, dtype=torch.int32),
-                "flip": torch.zeros(1, dtype=torch.int32)}
+        # anchors over the pyramid as the trunk makes it: the 7x7 stride-2 stem and the ceil-mode 3x3 stride-2 max
+        # pool give P2, every further level halves with (n - 1) // 2 + 1 (ceil(n / stride) is one more for widths
+        # such as 1985, the blob of a 370x1224 KITTI frame)
+        h, w, A = ((Ho - 1) // 2 - 1) // 2 + 1, ((Wo - 1) // 2 - 1) // 2 + 1, 0
+        for _ in OPS_CFG["FPN_FEAT_STRIDES"]:
+            A += h * w
+            h, w = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+        A *= len(OPS_CFG["ANCHOR_RATIOS"])
+        host = {"left_u8": torch.empty(B, H, W, 3, dtype=torch.uint8),
+                "right_u8": torch.empty(B, H, W, 3, dtype=torch.uint8),
+                "gt_classes": torch.zeros(B, N, dtype=torch.int32), "n_rows": torch.zeros(B, dtype=torch.int32),
+                "flip": torch.zeros(B, dtype=torch.int32)}
         for k, w in GT_ROW_FIELDS:
-            host[k] = torch.zeros(1, N, w, dtype=torch.float32)
+            host[k] = torch.zeros(B, N, w, dtype=torch.float32)
         self._host = {k: v.pin_memory() for k, v in host.items()}
         self._dev = {k: torch.zeros_like(v, device=device) for k, v in host.items()}
         self.left_u8, self.right_u8 = self._dev["left_u8"], self._dev["right_u8"]
@@ -610,32 +628,38 @@ class StepInputs(object):
         self.rows = {k: self._dev[k] for k in ("gt_classes",) + tuple(k for k, _ in GT_ROW_FIELDS)}
         f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
         i32 = lambda *s: torch.zeros(*s, dtype=torch.int32, device=device)
-        self.im_left, self.im_right = f(1, 3, Ho, Wo), f(1, 3, Ho, Wo)
-        self.gt = (f(1, 30, 5), f(1, 30, 5), f(1, 30, 5), f(1, 30, 5), f(1, 30, 6), i32(1))
-        self.shuffle_words, self.keys, self.words = i32(1, N), i32(1, R + MAX_NUM_GT_BOXES), i32(1, S)
-        self.rpn_keys, self.dropout_words = i32(1, A), i32(2, S, 2048)
-        # the index of a tensor here is its sb_random_words stream id
+        self.im_left, self.im_right = f(B, 3, Ho, Wo), f(B, 3, Ho, Wo)
+        self.gt = (f(B, 30, 5), f(B, 30, 5), f(B, 30, 5), f(B, 30, 5), f(B, 30, 6), i32(B))
+        self.shuffle_words, self.keys, self.words = i32(B, N), i32(B, R + MAX_NUM_GT_BOXES), i32(B, S)
+        self.rpn_keys, self.dropout_words = i32(B, A), i32(2, B * S, 2048)
+        # the index of a tensor here is its sb_random_words stream id (offset by 5 rank, Trainer.step_from_frames)
         self.word_tensors = (self.shuffle_words, self.keys, self.words, self.rpn_keys, self.dropout_words)
         self._copy_stream = torch.cuda.Stream(device)
         self._copied, self._consumed = torch.cuda.Event(), torch.cuda.Event()
 
-    def load(self, entry, left, right):
-        """fill the inputs from a roidb entry and its two uint8 [H,W,3] frames (numpy arrays or tensors): a host copy
-        into pinned memory, then non_blocking copies on the copy stream, which first waits until the step that last
-        read these buffers has finished.  The host waits only for the previous load's copies out of the pinned
-        buffers."""
+    def load(self, entries, frames, right=None):
+        """fill the inputs from B roidb entries and their B frame pairs [(left, right)] of uint8 [H,W,3] (numpy
+        arrays or tensors); load(entry, left, right) is the one-pair form.  A host copy into pinned memory, then
+        non_blocking copies on the copy stream, which first waits until the step that last read these buffers has
+        finished.  The host waits only for the previous load's copies out of the pinned buffers."""
+        if right is not None:
+            entries, frames = [entries], [(frames, right)]
+        B = self.batch
+        if len(entries) != B or len(frames) != B:
+            raise ValueError("%d entries and %d frame pairs for a StepInputs of %d pairs" % (len(entries), len(frames), B))
         self._copied.synchronize()
         h = self._host
-        n = int(len(entry["gt_classes"]))
         N = h["gt_classes"].shape[1]
-        if n > N:
-            raise ValueError("%d annotation rows exceed the capacity %d of this StepInputs" % (n, N))
-        h["left_u8"].copy_(torch.as_tensor(left))
-        h["right_u8"].copy_(torch.as_tensor(right))
-        h["gt_classes"][0, :n] = torch.as_tensor(np.asarray(entry["gt_classes"], np.int32))
-        for k, _ in GT_ROW_FIELDS:
-            h[k][0, :n] = torch.as_tensor(np.asarray(entry[k], np.float32))
-        h["n_rows"][0], h["flip"][0] = n, int(bool(entry.get("flipped", False)))
+        for b, (entry, (left, right)) in enumerate(zip(entries, frames)):
+            n = int(len(entry["gt_classes"]))
+            if n > N:
+                raise ValueError("%d annotation rows exceed the capacity %d of this StepInputs" % (n, N))
+            h["left_u8"][b].copy_(torch.as_tensor(left))
+            h["right_u8"][b].copy_(torch.as_tensor(right))
+            h["gt_classes"][b, :n] = torch.as_tensor(np.asarray(entry["gt_classes"], np.int32))
+            for k, _ in GT_ROW_FIELDS:
+                h[k][b, :n] = torch.as_tensor(np.asarray(entry[k], np.float32))
+            h["n_rows"][b], h["flip"][b] = n, int(bool(entry.get("flipped", False)))
         self._copy_stream.wait_event(self._consumed)
         with torch.cuda.stream(self._copy_stream):
             for k, v in h.items():
@@ -657,6 +681,36 @@ def epoch_order(n, generator):
     return torch.randperm(n, generator=generator).tolist()
 
 
+def epoch_batches(roidb, batch_size, generator, rank=0, world=1):
+    """The batches of one epoch that rank `rank` of `world` trains on, as lists of roidb indices.
+
+    batch_size 1: the batches of epoch_order(len(roidb), generator).  batch_size B > 1: every batch holds entries of
+    one frame shape, the documented difference from the reference (its aspect-ratio grouping, roidb.py:49-73, gives
+    every KITTI entry ratio 2, and its loader cannot stack blobs of different shapes): the entries are grouped by
+    (entry["height"], entry["width"]); within each group, in order of first appearance, a permutation is drawn and
+    cut into consecutive batches of B, a short tail dropped (as the reference drops int(train_size / bs)'s leftover);
+    then a permutation of all the batches is drawn.  Every rank draws the same epoch from the same generator state;
+    step k of rank r takes batch k world + r, so an epoch has floor(n_batches / world) steps."""
+    B, world = int(batch_size), int(world)
+    if B < 1 or world < 1 or not 0 <= rank < world:
+        raise ValueError("batch_size %d, rank %d of world %d" % (B, rank, world))
+    if B == 1:
+        batches = [[i] for i in epoch_order(len(roidb), generator)]
+    else:
+        groups = {}
+        for i, e in enumerate(roidb):
+            if "height" not in e or "width" not in e:
+                raise ValueError("roidb entry %d has no height / width: batches of %d pairs are grouped by frame "
+                                 "shape" % (i, B))
+            groups.setdefault((int(e["height"]), int(e["width"])), []).append(i)
+        cut = []
+        for members in groups.values():
+            perm = torch.randperm(len(members), generator=generator).tolist()
+            cut += [[members[j] for j in perm[k:k + B]] for k in range(0, len(perm) - B + 1, B)]
+        batches = [cut[j] for j in torch.randperm(len(cut), generator=generator).tolist()]
+    return [batches[k * world + rank] for k in range(len(batches) // world)]
+
+
 def lr_schedule(lr, start_epoch, epochs, lr_decay_step=5, lr_decay_gamma=0.1):
     """[(epoch, lr)] of trainval_net.py:184-191: the lr is multiplied by gamma at the start of every epoch with
     epoch % (lr_decay_step + 1) == 0"""
@@ -669,23 +723,30 @@ def lr_schedule(lr, start_epoch, epochs, lr_decay_step=5, lr_decay_gamma=0.1):
 
 
 def fit(trainer, roidb, frames, epochs, start_epoch=1, lr_decay_step=5, lr_decay_gamma=0.1, save_dir=None, log=print,
-        generator=None, target_size=600, max_rows=64, rgb_input=True):
-    """The training loop of trainval_net.py:183-258 at one stereo pair per step (minibatch.py:39-40) over
-    Trainer.step_from_frames, one CUDA graph per (frame shape, buffer set), two buffer sets per shape so that the
-    copy of the next entry overlaps the running step.
+        generator=None, target_size=600, max_rows=64, rgb_input=True, batch_size=1):
+    """The training loop of trainval_net.py:183-258 at `batch_size` stereo pairs per step and rank (the reference's
+    --bs, trainval_net.py:54-56) over Trainer.step_from_frames, two buffer sets per (frame shape) so that the copy of
+    the next batch overlaps the running step.  At trainer.world == 1 every (frame shape, buffer set) replays a CUDA
+    graph of its step; at world > 1 the steps run eagerly (the gradient all-reduce is a collective outside any graph).
 
     roidb: the reference's list of dicts (boxes_left, boxes_right, boxes_merge, dim_orien, kpts, gt_classes,
-    flipped; see append_flipped); frames(entry) -> (left, right) uint8 [H,W,3] arrays of the unflipped pair, decoded
-    by the caller (RGB unless rgb_input is False).  The epoch order is the reference sampler's, drawn from
-    `generator` (default: a torch.Generator seeded with trainer.seed, or continued from a loaded checkpoint); the lr
-    follows lr_schedule through trainer.set_lr.  Per step two lines go to `log` in the reference's format
-    (trainval_net.py:240-244); their numbers are copied to pinned memory behind an event and read one step late,
-    so the steady state has no device-wide synchronise.  With save_dir, trainer.checkpoint() is saved after every epoch as
-    stereo_rcnn_{epoch}_{last step}.pth (trainval_net.py:248-254).  To resume: trainer.load_checkpoint(ckpt), then
-    fit(..., start_epoch=ckpt["epoch"]).  -> [total loss of every step]"""
+    flipped; see append_flipped; with batch_size > 1 also the frame's height and width, as kitti_data.train_roidb sets
+    them); frames(entry) -> (left, right) uint8 [H,W,3] arrays of the unflipped pair, decoded by the caller (RGB
+    unless rgb_input is False).  The batches of an epoch are epoch_batches(roidb, batch_size, generator,
+    trainer.rank, trainer.world), drawn from `generator` (default: a torch.Generator seeded with trainer.seed, or
+    continued from a loaded checkpoint), the same on every rank; the lr follows lr_schedule through trainer.set_lr
+    (not scaled with the batch, as in the reference).  Per step rank 0 logs two lines in the reference's format
+    (trainval_net.py:240-244) with the losses averaged over the ranks (parallel.average_losses) and [iter k/n] counting
+    steps; the numbers are copied to pinned memory behind an event and read one step late, so the steady state has no
+    device-wide synchronise.  With save_dir, rank 0 saves trainer.checkpoint() after every epoch as
+    stereo_rcnn_{epoch}_{last step}.pth (trainval_net.py:248-254).  To resume, on every rank:
+    trainer.load_checkpoint(ckpt), then fit(..., start_epoch=ckpt["epoch"]).  -> [total loss of every step, averaged
+    over the ranks]"""
     import os
     from .engine import GraphRunner
+    from .parallel import average_losses
     dev = trainer.engine.device
+    world, rank, lead = trainer.world, trainer.rank, trainer.rank == 0
     gen = generator
     if gen is None:
         gen = torch.Generator()
@@ -698,38 +759,48 @@ def fit(trainer, roidb, frames, epochs, start_epoch=1, lr_decay_step=5, lr_decay
     stats_ev = [torch.cuda.Event() for _ in range(2)]
     totals = []
 
-    def load(entry):
-        left, right = frames(entry)
-        hw = tuple(int(v) for v in left.shape[:2])
+    def load(batch):
+        entries = [roidb[i] for i in batch]
+        pairs = [frames(e) for e in entries]
+        hw = tuple(int(v) for v in pairs[0][0].shape[:2])
         if hw not in slots:
-            slots[hw] = [StepInputs(hw, float(target_size) / float(min(hw)), dev, max_rows=max_rows,
-                                    rgb_input=rgb_input) for _ in range(2)]
+            slots[hw] = [StepInputs(hw, float(target_size) / float(min(hw)), dev, batch=batch_size,
+                                    max_rows=max_rows, rgb_input=rgb_input) for _ in range(2)]
             turn[hw] = 0
         inp = slots[hw][turn[hw]]
         turn[hw] ^= 1
-        inp.load(entry, left, right)
+        inp.load(entries, pairs)
         return inp
 
     def report(k, epoch, it, n, lr):
         stats_ev[k].synchronize()
         v = stats_host[k].tolist()
         totals.append(v[6])
+        if not lead:
+            return
         log("[epoch %2d][iter %4d/%4d] loss: %.4f, lr: %.2e" % (epoch, it, n, v[6], lr))
         log("\t\t\trpn_cls: %.4f, rpn_box_left_right: %.4f, rcnn_cls: %.4f, rcnn_box_left_right %.4f,dim_orien %.4f, "
             "kpts %.4f" % tuple(v[:6]))
 
-    n = len(roidb)
     for epoch, lr in lr_schedule(trainer.lr_value, start_epoch, epochs, lr_decay_step, lr_decay_gamma):
         if lr != trainer.lr_value:
             trainer.set_lr(lr)
-        order = epoch_order(n, gen)
-        nxt = load(roidb[order[0]])
-        for it, idx in enumerate(order):
+        order = epoch_batches(roidb, batch_size, gen, rank, world)
+        n = len(order)
+        if n == 0:
+            raise ValueError("an epoch of %d entries has no step of %d pairs on each of %d ranks"
+                             % (len(roidb), batch_size, world))
+        nxt = load(order[0])
+        for it in range(n):
             inp = nxt
             if it + 1 < n:
-                nxt = load(roidb[order[it + 1]])
+                nxt = load(order[it + 1])
             with torch.no_grad():
-                if id(inp) not in runners:
+                if world > 1:
+                    out = trainer.step_from_frames(inp)
+                    avg = average_losses(torch.cat((out[0], out[1])), world, trainer.dist)
+                    out = (avg[:6], avg[6:])
+                elif id(inp) not in runners:
                     # the first step on a buffer set runs eagerly (it creates the workspaces a capture needs); the
                     # capture that follows launches nothing
                     out = trainer.step_from_frames(inp)
@@ -746,7 +817,7 @@ def fit(trainer, roidb, frames, epochs, start_epoch=1, lr_decay_step=5, lr_decay
                 report(1 - k, epoch, it - 1, n, lr)
         report((n - 1) % 2, epoch, n - 1, n, lr)
         trainer.epoch, trainer.sampler_state = epoch + 1, gen.get_state()
-        if save_dir is not None:
+        if save_dir is not None and lead:
             name = os.path.join(save_dir, "stereo_rcnn_%d_%d.pth" % (epoch, n - 1))
             torch.save(trainer.checkpoint(), name)
             log("save model: %s" % name)

@@ -80,7 +80,7 @@ def run(args):
         step_graph = timed(r_step, args.steps, args.warmup)
         many = max(args.steps * 10, 200)
         pair_ms = timed(lambda: ops.prep_stereo_pair(inp.left_u8, inp.right_u8, SCALE, inp.flip, True,
-                                                     out=(inp.im_left[0], inp.im_right[0])), many, 10)
+                                                     out=(inp.im_left, inp.im_right)), many, 10)
 
         def fills():
             for sid, t in enumerate(inp.word_tensors):
@@ -92,8 +92,8 @@ def run(args):
         def replaced():
             for t in inp.word_tensors[1:]:
                 t.copy_(train.random_words(t.shape, dev))
-            ops.prep_image(inp.left_u8, SCALE, True, out=inp.im_left[0])
-            ops.prep_image(inp.right_u8, SCALE, True, out=inp.im_right[0])
+            ops.prep_image(inp.left_u8[0], SCALE, True, out=inp.im_left[0])
+            ops.prep_image(inp.right_u8[0], SCALE, True, out=inp.im_right[0])
         replaced_ms = timed(replaced, many, 10)
         skipped, steps_taken = int(tr.skipped.item()), int(tr.step_count.item())
     n_words = sum(t.numel() for t in inp.word_tensors)
