@@ -24,6 +24,13 @@
 //     the TMA producer.  One mbarrier ring (full / empty) of stages sized so that nearly all shared memory holds
 //     operands (4 stages of 48 KB for 256-wide tiles, 6 of 32 KB for 128-wide ones); the producer runs ahead into
 //     the next tile while the consumers finish the epilogue of the current one.
+//   * ping-pong schedule (fp16 operands, register epilogue, tiles of at most 128 columns -- 64 with the upsample-add
+//     -- and a launch where some CTA gets a second tile): the CTA's j-th tile belongs to warpgroup j & 1, which
+//     issues two m64nNk16 wgmma per k16 (one per 64-row half of the A stage) and owns all 128 rows' accumulators.  The mainloops take turns (a pair of
+//     mbarriers: a warpgroup starts a tile once the other has issued its previous tile's last K-step), so each
+//     tile's register epilogue runs under the other warpgroup's MMAs.  Each stage is consumed by one warpgroup; it
+//     finds the ring position of its tile from the K-steps before it, j * num_k_blocks.  Every output element sums
+//     the same K-steps in the same order as under the cooperative schedule, so the results are bit-identical.
 //   * fused epilogue straight out of the accumulator registers: folded frozen-BN scale/shift or bias, residual add,
 //     FPN bilinear (align_corners) upsample-add, ReLU, the TF32 store modes, fp32 and/or fp16 ("twin") stores with
 //     arbitrary n/h/w strides and channel offset (RPN L|R concat, deconv scatter).  All loads of a column step (both
@@ -43,7 +50,8 @@
 //     32-wide: 7 x 20 KB + 2 x 3 x 12 KB).  The TF32 mode and the data-gradient variants keep the register epilogue.
 //   * programmatic dependent launch: the prologue (barrier init, descriptor prefetch) overlaps the previous
 //     kernel's tail; dependents are released after the CTA's last operand loads are issued.
-//   * optional per-CTA phase trace (sb_conv_trace) for tools/conv_trace.py.
+//   * optional per-CTA phase trace (sb_conv_trace) for tools/conv_trace.py: timestamps, the schedule and the tiles
+//     each consumer warpgroup computed.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <stdlib.h>
@@ -86,7 +94,11 @@ __device__ __forceinline__ unsigned long long gtimer() {
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t) :: "memory");
     return t;
 }
+// Trace words of a CTA: [0..5] %globaltimer and [8..13] clock64 at entry, after griddepcontrol.wait, first operand
+// stage landed, last operand load issued, first tile's epilogue done, exit; [6] SM id; [7] schedule (0 cooperative,
+// 1 ping-pong); [14 + g] tiles computed by consumer warpgroup g (counted once per tile, outside the K loop).
 constexpr int kTraceWords = 16, kTraceCtas = 304;
+constexpr int kTraceSched = 7, kTraceTiles = 14;
 
 // TMA residual epilogue (fp16-operand forward with a residual): per consumer warpgroup, a ring of epi_slots(BLOCK_N)
 // slots, each one 32-column chunk of the warpgroup's 64 tile rows: an fp32 box [64 rows][32 columns] (residual in,
@@ -98,21 +110,30 @@ constexpr int kResThreads = kThreads + 32 * kResProducerWarps;
 constexpr bool tma_epilogue(bool has_res, bool in16, bool mask) { return has_res && in16 && !mask; }
 constexpr int epi_slots(int block_n) { return block_n == 128 ? 4 : 3; }
 constexpr int conv_threads(bool stem, bool tma_epi) { return stem ? kStemThreads : tma_epi ? kResThreads : kThreads; }
-
-// operand stages, then (slots > 0) both warpgroups' epilogue rings, the 1024-byte alignment pad and the mbarriers
-// (operand ring, epilogue rings, the residual producers' start)
-constexpr size_t conv_smem(int block_n, int stages, int slots) {
-    return (size_t)stages * (BLOCK_M * kRowBytes + block_n * kRowBytes) + (size_t)2 * slots * kSlotBytes + 1024 +
-           (2 * stages + 4 * slots + 1) * 8;
+// instantiations that have a ping-pong twin: fp16 operands, the epilogue runs from registers, and a warpgroup's
+// 128 x BLOCK_N accumulators and its four rows' epilogue state fit the register budget without spills -- 168 per
+// thread at 288 threads and one CTA per SM (nine warps on four 16K-register SM sub-partitions).  At 128 columns the
+// upsample-add epilogue does not (2.4 KB of spill stores), so that one stays cooperative.
+constexpr bool pingpong_ok(int block_n, bool has_res, bool has_up, bool in16, bool stem, bool mask) {
+    return in16 && !tma_epilogue(has_res, in16, mask) && !stem && !mask && block_n <= (has_up ? 64 : 128);
 }
 
-template <int BLOCK_N, int kStages, bool HAS_RES, bool HAS_UP, bool IN16, bool STEM = false, bool MASK = false>
+// operand stages, then (slots > 0) both warpgroups' epilogue rings, the 1024-byte alignment pad and the mbarriers
+// (operand ring, epilogue rings, the residual producers' start, the two ping-pong turns)
+constexpr size_t conv_smem(int block_n, int stages, int slots) {
+    return (size_t)stages * (BLOCK_M * kRowBytes + block_n * kRowBytes) + (size_t)2 * slots * kSlotBytes + 1024 +
+           (2 * stages + 4 * slots + 3) * 8;
+}
+
+template <int BLOCK_N, int kStages, bool HAS_RES, bool HAS_UP, bool IN16, bool STEM = false, bool MASK = false,
+          bool PP = false>
 __global__ void __launch_bounds__(conv_threads(STEM, tma_epilogue(HAS_RES, IN16, MASK)), 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                const __grid_constant__ CUtensorMap map_r, const __grid_constant__ CUtensorMap map_o,
                const __grid_constant__ CUtensorMap map_o16, const TcParams p) {
     static_assert(!STEM || (IN16 && !HAS_RES && !HAS_UP), "stem variant");
     static_assert(!MASK || (IN16 && !HAS_UP && !STEM), "mask variant");
+    static_assert(!PP || pingpong_ok(BLOCK_N, HAS_RES, HAS_UP, IN16, STEM, MASK), "ping-pong variant");
     constexpr bool kTmaEpi = tma_epilogue(HAS_RES, IN16, MASK);
     static_assert(!kTmaEpi || BLOCK_N <= 128, "residual layers use tiles of at most 128 columns");
     constexpr uint32_t kABytes = BLOCK_M * kRowBytes, kBBytes = BLOCK_N * kRowBytes;
@@ -130,6 +151,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     uint64_t* slot_full = empty + kStages;         // [2][kSlots]: the chunk's residual box has landed
     uint64_t* slot_empty = slot_full + 2 * kSlots; // [2][kSlots]: the chunk's output stores have read the slot
     uint64_t* res_go = slot_empty + 2 * kSlots;    // the first tile's first operand loads are issued
+    uint64_t* turn = res_go + 1;                   // [2] (PP): warpgroup g may start its next tile's K loop
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const sb_conv_desc& d = p.d;
@@ -138,16 +160,23 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         unsigned smid;
         asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
         tr[0] = gtimer(); tr[8] = clock64(); tr[6] = smid;
+        tr[kTraceSched] = PP ? 1 : 0;
+        tr[kTraceTiles] = tr[kTraceTiles + 1] = 0;     // counted below by the warpgroups' thread 0
     }
     if (warp == kProducerWarp && lane == 0) {
         if (!STEM) prefetch_tmap(&map_a);
         prefetch_tmap(&map_b);
         if (kTmaEpi) prefetch_tmap(&map_r);
         // STEM: a stage is full when the weight tile has landed (1 expect_tx arrival) and the gather threads have
-        // written their patch rows.  A stage is empty when every consumer warp's MMAs on it have completed.
+        // written their patch rows.  A stage is empty when the MMAs on it of every consumer warp that reads it
+        // (all eight; PP: the four of the tile's warpgroup) have completed.
         for (int i = 0; i < kStages; ++i) {
             mbar_init(&full[i], STEM ? 1 + 32 * kStemGatherWarps : 1);
-            mbar_init(&empty[i], kConsumerWarps);
+            mbar_init(&empty[i], PP ? kConsumerWarps / 2 : kConsumerWarps);
+        }
+        if (PP) {
+            mbar_init(&turn[0], kConsumerWarps / 2);     // lane 0 of each warp of the other warpgroup
+            mbar_init(&turn[1], kConsumerWarps / 2);
         }
         for (int i = 0; i < 2 * kSlots; ++i) {
             mbar_init(&slot_full[i], 1);         // the residual producer's expect_tx arrival
@@ -318,15 +347,20 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         }
     } else {
         // ===================== consumers: wgmma main loop + epilogue (warps 0..7) =====================
-        // Warpgroup wg computes rows 64*wg .. 64*wg+63 of the tile against all BLOCK_N columns.  This thread holds
-        // rows r_lo and r_lo + 8, columns 8*j + cq + {0,1} for j < BLOCK_N/8 (wgmma.cuh: fragment layout).
+        // Cooperative: warpgroup wg computes rows 64*wg .. 64*wg+63 of every tile against all BLOCK_N columns; this
+        // thread holds rows r_lo and r_lo + 8, columns 8*j + cq + {0,1} for j < BLOCK_N/8 (wgmma.cuh: fragment
+        // layout).  PP: warpgroup wg computes all 128 rows of the CTA's tiles j = wg, wg + 2, ..., as two 64-row
+        // halves; this thread holds rows r_lo, r_lo + 8, r_lo + 64 and r_lo + 72 (accumulators of the second half at
+        // kAcc + ...).
         const int wg = warp >> 2;
-        const int r_lo = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+        constexpr int kHalves = PP ? 2 : 1;
+        constexpr int kRows = 2 * kHalves;
+        const int r_lo = (PP ? 0 : 64 * wg) + 16 * (warp & 3) + (lane >> 2);
         const int cq = 2 * (lane & 3);
-        constexpr int kAcc = BLOCK_N / 2;
-        float acc[kAcc];
+        constexpr int kAcc = BLOCK_N / 2;      // per 64-row half
+        float acc[kHalves * kAcc];
 #pragma unroll
-        for (int i = 0; i < kAcc; ++i) acc[i] = 0.f;
+        for (int i = 0; i < kHalves * kAcc; ++i) acc[i] = 0.f;
         float rh = 0.f, rw = 0.f;
         if (HAS_UP) {
             rh = d.Ho > 1 ? __fdiv_rn((float)(d.UH - 1), (float)(d.Ho - 1)) : 0.f;
@@ -342,23 +376,42 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         int slot = 0, held = -1;
         uint32_t sphase = 0;
         const bool store_thread = (threadIdx.x & 127) == 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        // the CTA's jt-th tile (PP: jt = wg, wg + 2, ...)
+        for (int tile = blockIdx.x + (PP ? wg * (int)gridDim.x : 0), jt = PP ? wg : 0; tile < num_tiles;
+             tile += (PP ? 2 : 1) * gridDim.x, jt += PP ? 2 : 1) {
             const int mt = tile / p.num_n_tiles, nt = tile - mt * p.num_n_tiles;
+            if (PP) {
+                // ring position of the tile's first K-step: the tiles before it took jt * num_k_blocks stages, the
+                // last of them by the other warpgroup (num_k_blocks need not divide kStages)
+                const unsigned ks = (unsigned)jt * (unsigned)p.num_k_blocks;
+                stage = (int)(ks % kStages);
+                phase = (ks / kStages) & 1u;
+                // wait for the turn: the other warpgroup has issued tile jt - 1's last K-step, so every K-step before
+                // this tile has landed (no `full` wait below is a phase behind) and the two mainloops alternate
+                if (jt > 0) mbar_wait(&turn[wg], ((unsigned)(jt - 1) >> 1) & 1u);
+            }
             int prev = 0;
             for (int kb = 0; kb < p.num_k_blocks; ++kb) {
                 mbar_wait(&full[stage], phase);
                 if (tr && threadIdx.x == 0 && kb == 0 && tile == (int)blockIdx.x) { tr[2] = gtimer(); tr[10] = clock64(); }
                 const uint32_t sa = smem_u32(smem + stage * kStageBytes);
-                const uint64_t da = make_smem_desc(sa + wg * (kABytes / 2)), db = make_smem_desc(sa + kABytes);
+                const uint64_t db = make_smem_desc(sa + kABytes);
 #pragma unroll
-                for (int i = 0; i < kAcc; ++i) reg_fence(acc[i]);
+                for (int i = 0; i < kHalves * kAcc; ++i) reg_fence(acc[i]);
                 wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < 4; ++k)    // advance 32 bytes (16 fp16 / 8 tf32) inside the 128-byte swizzle row
-                    Wgmma<BLOCK_N, IN16>::mma(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) != 0);
+                for (int k = 0; k < 4; ++k) {  // advance 32 bytes (16 fp16 / 8 tf32) inside the 128-byte swizzle row
+#pragma unroll
+                    for (int hf = 0; hf < kHalves; ++hf) {
+                        const uint64_t da = make_smem_desc(sa + (PP ? hf : wg) * (kABytes / 2));
+                        Wgmma<BLOCK_N, IN16>::mma(acc + hf * kAcc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2),
+                                                  (kb | k) != 0);
+                    }
+                }
                 wgmma_commit();
 #pragma unroll
-                for (int i = 0; i < kAcc; ++i) reg_fence(acc[i]);
+                for (int i = 0; i < kHalves * kAcc; ++i) reg_fence(acc[i]);
+                if (PP && kb == p.num_k_blocks - 1 && lane == 0) mbar_arrive(&turn[wg ^ 1]);     // pass the turn
                 // keep one K-step of MMAs in flight: the previous step's are complete, its stage may be refilled
                 wgmma_wait<1>();
                 if (kb > 0 && lane == 0) mbar_arrive(&empty[prev]);
@@ -376,7 +429,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             }
             wgmma_wait<0>();
 #pragma unroll
-            for (int i = 0; i < kAcc; ++i) reg_fence(acc[i]);
+            for (int i = 0; i < kHalves * kAcc; ++i) reg_fence(acc[i]);
             if (lane == 0) mbar_arrive(&empty[prev]);
 
             if constexpr (kTmaEpi) {
@@ -439,16 +492,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                 }
             } else {
                 // ---- epilogue from registers: per row {output offset, residual row, upsample source + weights}, then
-                // per column pair
-                long long ooff[2];
-                bool valid[2];
-                long long rrow[2];
-                int uoff[2];
-                float uly[2], ulx[2];
-                bool by[2], bx[2];
+                // per column pair.  Row h is r_lo + 8 * (h & 1) + 64 * (h >> 1), its accumulators at
+                // (h >> 1) * kAcc + 4 * j + 2 * (h & 1) + {0, 1}.
+                long long ooff[kRows];
+                bool valid[kRows];
+                long long rrow[kRows];
+                int uoff[kRows];
+                float uly[kRows], ulx[kRows];
+                bool by[kRows], bx[kRows];
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int row = r_lo + 8 * h;
+                for (int h = 0; h < kRows; ++h) {
+                    const int row = r_lo + 8 * (h & 1) + 64 * (h >> 1);
                     int n_img, ho, wo;
                     long long m = 0;
                     if (p.patch) {
@@ -487,13 +541,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                     const int c = nt * BLOCK_N + 8 * j + cq;      // Cout % 4 == 0: c < Cout implies c + 1 < Cout
                     const bool cv = c < d.Cout;
                     const int cs = cv ? c : 0;                    // past Cout: any in-bounds column, never stored
-                    // every load of the column step, for both rows, is issued before its first store (addresses of
+                    // every load of the column step, for all rows, is issued before its first store (addresses of
                     // invalid rows and columns are clamped into the tensors instead of branching around the loads)
                     const float2 sc = d.scale ? __ldg(reinterpret_cast<const float2*>(d.scale + cs)) : make_float2(1.f, 1.f);
                     const float2 sh = d.shift ? __ldg(reinterpret_cast<const float2*>(d.shift + cs)) : make_float2(0.f, 0.f);
-                    float2 rv[2], ua[2], ub[2], ug[2], uh[2];
+                    float2 rv[kRows], ua[kRows], ub[kRows], ug[kRows], uh[kRows];
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
+                    for (int h = 0; h < kRows; ++h) {
                         if (HAS_RES) rv[h] = __ldg(reinterpret_cast<const float2*>(d.residual + rrow[h] + cs));
                         if (HAS_UP) {
                             const float* u00 = d.up_src + uoff[h] + cs;
@@ -506,10 +560,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                         }
                     }
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
+                    for (int h = 0; h < kRows; ++h) {
                         if (!cv || !valid[h]) continue;
-                        float x0 = fmaf(acc[4 * j + 2 * h], sc.x, sh.x);
-                        float x1 = fmaf(acc[4 * j + 2 * h + 1], sc.y, sh.y);
+                        const int ai = (h >> 1) * kAcc + 4 * j + 2 * (h & 1);
+                        float x0 = fmaf(acc[ai], sc.x, sh.x);
+                        float x1 = fmaf(acc[ai + 1], sc.y, sh.y);
                         if (HAS_RES) {
                             float2 r = rv[h];
                             if (res_biased) { r.x = sb_unbias_tf32(r.x); r.y = sb_unbias_tf32(r.y); }
@@ -539,6 +594,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                 }
             }
             if (tr && threadIdx.x == 0 && tile == (int)blockIdx.x) { tr[4] = gtimer(); tr[12] = clock64(); }
+            if (tr && store_thread) atomicAdd(tr + kTraceTiles + wg, 1ull);
         }
         if (kTmaEpi && (threadIdx.x & 127) == 0) bulk_wait<0>();     // the last tile's stores have completed
     }
@@ -632,12 +688,22 @@ struct TcMaps {
     CUtensorMap a, b, r, o, o16;
 };
 
-template <int BN, int ST, bool RES, bool UP, bool IN16, bool STEM = false, bool MASK = false>
+// PP: the ping-pong schedule.  An instantiation that has a ping-pong twin runs it when some CTA gets a second tile.
+// With one tile per CTA there is no other tile's epilogue to hide, and a warpgroup alone would run all 128 rows'.
+
+template <int BN, int ST, bool RES, bool UP, bool IN16, bool STEM = false, bool MASK = false, bool PP = false>
 int launch_t(const TcMaps& m, const TcParams& p, cudaStream_t st) {
+    const int tiles = p.num_m_tiles * p.num_n_tiles;
+    int slots = sb_num_sms();
+    if (p.d.max_ctas > 0 && p.d.max_ctas < slots) slots = p.d.max_ctas;
+    const int grid = tiles < slots ? tiles : slots;
+    if constexpr (!PP && pingpong_ok(BN, RES, UP, IN16, STEM, MASK)) {
+        if (tiles > grid) return launch_t<BN, ST, RES, UP, IN16, STEM, MASK, true>(m, p, st);
+    }
     constexpr bool tma_epi = tma_epilogue(RES, IN16, MASK);
     constexpr size_t smem = conv_smem(BN, ST, tma_epi ? epi_slots(BN) : 0);
     static_assert(smem <= 227 * 1024, "smem budget");
-    auto kern = conv_tc_kernel<BN, ST, RES, UP, IN16, STEM, MASK>;
+    auto kern = conv_tc_kernel<BN, ST, RES, UP, IN16, STEM, MASK, PP>;
     static bool attr_done[kSbMaxDevices] = {false};
     bool& attr = attr_done[sb_cur_device()];
     if (!attr) {
@@ -645,10 +711,6 @@ int launch_t(const TcMaps& m, const TcParams& p, cudaStream_t st) {
         if (e != cudaSuccess) return (int)e;
         attr = true;
     }
-    const int tiles = p.num_m_tiles * p.num_n_tiles;
-    int slots = sb_num_sms();
-    if (p.d.max_ctas > 0 && p.d.max_ctas < slots) slots = p.d.max_ctas;
-    const int grid = tiles < slots ? tiles : slots;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(conv_threads(STEM, tma_epi));
