@@ -242,8 +242,79 @@ class _EvalSlot(object):
         return out
 
 
+def _eval_block(pipe, entries, ks, frames, calib, inflight, use_graph, target_size, rgb_input, states, emit):
+    """evaluate's slot loop over the entries[k] of the range `ks`: emit(k, final, t_cam2_cam0_x) once per entry, in
+    entry order, with the image's solved rows (pinned host memory that the slot's next step overwrites).  states: the
+    {(frame shape, slot): _EvalSlot} to use and fill.  -> the number of graphs captured"""
+    pending = [None] * inflight                  # per slot: (entry index, _EvalSlot, t_cam2_cam0_x)
+    graphs = [0]
+
+    def load(k):
+        left, right = frames(entries[k])
+        hw = (int(left.shape[0]), int(left.shape[1]))
+        key = (hw, k % inflight)
+        if key not in states:
+            states[key] = _EvalSlot(pipe, hw, target_size, rgb_input)
+        st = states[key]
+        c = calib(entries[k])
+        st.inp.load(left, right, c)
+        return st, c.t_cam2_cam0_x
+
+    def launch(st):
+        with torch.cuda.stream(st.stream), torch.no_grad(), ops.workspace_owner(st.ws):
+            if not use_graph or st.runner is None:
+                st.step(pipe)                    # eager; the first step on a slot also creates its workspaces
+                if use_graph:
+                    from .engine import GraphRunner
+                    st.runner = GraphRunner(lambda: st.step(pipe), [], warmup=0)
+                    graphs[0] += 1
+            else:
+                st.inp.ready()
+                st.runner()
+                st.inp.release()
+            st.done.record(st.stream)
+
+    def finish(p):
+        k, st, t_x = p
+        st.done.synchronize()
+        emit(k, st.final_h[:int(st.n_h[0])], t_x)
+
+    ks = list(ks)
+    nxt = load(ks[0]) if ks else None
+    for j, k in enumerate(ks):
+        st, t_x = nxt
+        if pending[k % inflight] is not None:    # entry k - inflight: read before this slot's buffers are reused
+            finish(pending[k % inflight])
+        launch(st)
+        pending[k % inflight] = (k, st, t_x)
+        if j + 1 < len(ks):
+            nxt = load(ks[j + 1])                # host reads + H2D of the next entry overlap this step
+    end = ks[-1] + 1 if ks else 0
+    for j in range(inflight):                    # the last ones, in entry order
+        p = pending[(end + j) % inflight]
+        if p is not None:
+            finish(p)
+    return graphs[0]
+
+
+def _agree(err, world, dist):
+    """every rank raises the first rank's refusal, or none does: no rank is left waiting in a collective"""
+    errs = [None] * world
+    dist.all_gather_object(errs, err)
+    return next((e for e in errs if e is not None), None)
+
+
+def _log_summary(summary, log, ranks=1):
+    log("evaluate: %d images, %d lines in %d files, %d graphs%s" % (
+        summary["images"], summary["lines"], summary["files"], summary["graphs"],
+        " on %d ranks" % ranks if ranks > 1 else ""))
+    if "ap" in summary:
+        log("evaluate: Car AP|R11 (easy, moderate, hard) 2D %s, AOS %s, BEV %s, 3D %s at IoU 0.7" % tuple(
+            "/".join("%.2f" % v for v in summary["ap"][m][0.7][:, 0]) for m in ("bbox", "aos", "bev", "3d")))
+
+
 def evaluate(pipe, entries, frames, calib, result_dir, inflight=1, use_graph=True, target_size=600, rgb_input=True,
-             name=None, log=print, empty_files=False, labels=None):
+             name=None, log=print, empty_files=False, labels=None, world=1, dist=None, slots=None):
     """The test loop of test_net.py:118-335 over a split: per entry the frames and the calibration, forward, decode,
     per-class NMS, infer_boundary, solve_x_y_z_theta_from_kpt, align_parallel, solve_x_y_theta_from_kpt (all in
     StereoPipeline.step_from_frames), then write_detection_results' lines (kitti_utils.py:440-460) in
@@ -267,83 +338,115 @@ def evaluate(pipe, entries, frames, calib, result_dir, inflight=1, use_graph=Tru
     labels(entry) -> the image's KITTI label file (a path or its text): when given, the lines written for each image
     are scored against it (kitti_eval.KittiEval, on the device, after the loop), images without a detection included,
     and summary["ap"] holds KittiEval.result() -- the Car AP of exactly the files written.
-    -> dict(images, lines, files, graphs, write_s: host seconds spent formatting and writing the files[, ap])"""
+
+    world > 1 with dist (torch.distributed, this process's rank of `world`): rank r runs the same loop over its
+    contiguous block parallel.shard_pairs(len(entries), r, world) and formats its own lines; after the loop one
+    gather_object brings every rank's (entry index, lines) to rank 0, which alone creates result_dir/data, writes the
+    files in entry order and scores the whole split, then broadcasts the summary, so every rank returns the same one
+    and ranks need not share a filesystem.  The files and the scores are those of the same split on one GPU.  The
+    refusals above are decided before any work (the result directory by rank 0) and raised on every rank.  A rank
+    whose block is empty takes part in the collectives and evaluates nothing.
+
+    slots: a dict that keeps the (frame shape, slot) inputs, workspaces and graphs between calls; later calls with the
+    same dict, pipeline, target_size and rgb_input replay those graphs instead of capturing new ones.  Its graphs read
+    the pipeline's packed weights when they run, so they see what eng.refresh_weights writes there in between (the
+    kept slots' streams first wait for the work enqueued on the current stream).
+    -> dict(images, lines, files, graphs: graphs captured in this call, write_s: host seconds spent formatting and
+    writing the files[, ap, score_s: host seconds spent scoring]); at world > 1 images, lines, files and graphs are
+    totals over the ranks, write_s is rank 0's writing after the gather (each rank formats its lines in its loop),
+    and rank_images and loop_s (each rank's images and seconds in its loop) and gather_s (rank 0's seconds in the
+    gather, waiting for the slowest rank included) are added"""
+    sharded = int(world) > 1 and dist is not None
+    rank = int(dist.get_rank()) if sharded else 0
     data_dir = os.path.join(result_dir, "data")
-    if glob.glob(os.path.join(data_dir, "*.txt")):
-        raise FileExistsError("%s already holds result files; evaluate writes into an empty directory" % data_dir)
-    if inflight < 1:
-        raise ValueError("inflight must be >= 1")
-    if use_graph and pipe.eng.forks:
-        raise ValueError("evaluate captures its graphs from a pipeline built with throughput=True")
-    os.makedirs(data_dir, exist_ok=True)
+    err = None
+    if rank == 0 and glob.glob(os.path.join(data_dir, "*.txt")):
+        err = FileExistsError("%s already holds result files; evaluate writes into an empty directory" % data_dir)
+    elif inflight < 1:
+        err = ValueError("inflight must be >= 1")
+    elif use_graph and pipe.eng.forks:
+        err = ValueError("evaluate captures its graphs from a pipeline built with throughput=True")
+    if sharded:
+        err = _agree(err, int(world), dist)
+    if err is not None:
+        raise err
+    if rank == 0:
+        os.makedirs(data_dir, exist_ok=True)
     name = name or (lambda e: e["image_id"])
-    states = {}
-    pending = [None] * inflight                  # per slot: (entry index, _EvalSlot, t_cam2_cam0_x, file stem)
+    states = {} if slots is None else slots.setdefault((id(pipe), float(target_size), bool(rgb_input)), {})
+    for st in states.values():                   # kept slots run after what the caller enqueued (a weight refresh)
+        st.stream.wait_stream(torch.cuda.current_stream(pipe.dev))
     summary = dict(images=0, lines=0, files=0, graphs=0, write_s=0.0)
+    texts = {}
     scorer = None
-    if labels is not None:
+    if labels is not None and rank == 0:
         from .kitti_eval import KittiEval
         scorer = KittiEval(pipe.dev)
 
-    def load(k):
-        left, right = frames(entries[k])
-        hw = (int(left.shape[0]), int(left.shape[1]))
-        key = (hw, k % inflight)
-        if key not in states:
-            states[key] = _EvalSlot(pipe, hw, target_size, rgb_input)
-        st = states[key]
-        c = calib(entries[k])
-        st.inp.load(left, right, c)
-        return st, c.t_cam2_cam0_x
-
-    def launch(st):
-        with torch.cuda.stream(st.stream), torch.no_grad(), ops.workspace_owner(st.ws):
-            if not use_graph or st.runner is None:
-                st.step(pipe)                    # eager; the first step on a slot also creates its workspaces
-                if use_graph:
-                    from .engine import GraphRunner
-                    st.runner = GraphRunner(lambda: st.step(pipe), [], warmup=0)
-                    summary["graphs"] += 1
-            else:
-                st.inp.ready()
-                st.runner()
-                st.inp.release()
-            st.done.record(st.stream)
-
-    def finish(p):
-        k, st, t_x, stem = p
-        st.done.synchronize()
-        t0 = time.perf_counter()
-        n = int(st.n_h[0])
-        lines = ops.kitti_result_lines(st.final_h[:n], t_x)
+    def write(k, lines):
         if lines or empty_files:
-            with open(os.path.join(data_dir, stem + ".txt"), "w") as f:
+            with open(os.path.join(data_dir, str(name(entries[k])) + ".txt"), "w") as f:
                 f.write("".join(lines))
             summary["files"] += 1
-        summary["write_s"] += time.perf_counter() - t0
-        if scorer is not None:
-            scorer.add(labels(entries[k]), "".join(lines))
         summary["images"] += 1
         summary["lines"] += len(lines)
 
+    def score(k, lines):
+        t0 = time.perf_counter()
+        scorer.add(labels(entries[k]), "".join(lines))
+        summary["score_s"] = summary.get("score_s", 0.0) + time.perf_counter() - t0
+
+    def emit(k, final, t_x):
+        t0 = time.perf_counter()
+        lines = ops.kitti_result_lines(final, t_x)
+        if sharded:                              # formatted here, written by rank 0 after the gather
+            texts[k] = lines
+            return
+        write(k, lines)
+        summary["write_s"] += time.perf_counter() - t0
+        if scorer is not None:
+            score(k, lines)
+
     n = len(entries)
-    nxt = load(0) if n else None
-    for k in range(n):
-        st, t_x = nxt
-        if pending[k % inflight] is not None:    # entry k - inflight: read before this slot's buffers are reused
-            finish(pending[k % inflight])
-        launch(st)
-        pending[k % inflight] = (k, st, t_x, str(name(entries[k])))
-        if k + 1 < n:
-            nxt = load(k + 1)                    # host reads + H2D of the next entry overlap this step
-    for j in range(inflight):                    # the last ones, in entry order
-        p = pending[(n + j) % inflight]
-        if p is not None:
-            finish(p)
-    log("evaluate: %d images, %d lines in %d files, %d graphs" % (summary["images"], summary["lines"],
-                                                                 summary["files"], summary["graphs"]))
+    b, e = parallel.shard_pairs(n, rank, int(world)) if sharded else (0, n)
+    t0 = time.perf_counter()
+    try:
+        summary["graphs"] = _eval_block(pipe, entries, range(b, e), frames, calib, inflight, use_graph, target_size,
+                                        rgb_input, states, emit)
+    finally:
+        if slots is None:
+            # a slot and its graph refer to each other: freed here, not by the garbage collector during a later
+            # capture, where releasing the slot's pinned buffers (a CUDA event record) would invalidate that capture
+            for st in states.values():
+                st.runner = None
+    if sharded:
+        t1 = time.perf_counter()
+        parts = [None] * int(world) if rank == 0 else None
+        dist.gather_object((texts, summary["graphs"], t1 - t0), parts, dst=0)
+        if rank == 0:
+            summary["gather_s"] = time.perf_counter() - t1
+            for part, _g, _t in parts:
+                texts.update(part)
+            t0 = time.perf_counter()
+            for k in range(n):
+                write(k, texts[k])
+            summary["write_s"] = time.perf_counter() - t0
+            summary["graphs"] = sum(g for _p, g, _t in parts)
+            summary["rank_images"] = [len(p) for p, _g, _t in parts]
+            summary["loop_s"] = [t for _p, _g, t in parts]
+            if scorer is not None:
+                for k in range(n):
+                    score(k, texts[k])
+        else:
+            summary = None
     if scorer is not None and n:
+        t0 = time.perf_counter()
         summary["ap"] = scorer.result()
-        log("evaluate: Car AP|R11 (easy, moderate, hard) 2D %s, AOS %s, BEV %s, 3D %s at IoU 0.7" % tuple(
-            "/".join("%.2f" % v for v in summary["ap"][m][0.7][:, 0]) for m in ("bbox", "aos", "bev", "3d")))
+        summary["score_s"] += time.perf_counter() - t0
+    if sharded:
+        out = [summary]
+        dist.broadcast_object_list(out, src=0)
+        summary = out[0]
+    if rank == 0:
+        _log_summary(summary, log, int(world) if sharded else 1)
     return summary

@@ -488,6 +488,7 @@ class Trainer(object):
         # step_from_frames: the key of the step's random words and the device-side count of the steps taken
         self.seed, self.step_count = int(seed), torch.zeros(1, dtype=torch.int64, device=dev)
         self.epoch, self.sampler_state = 1, None     # the next epoch of fit and the state of its host generator
+        self.val_summaries = {}                      # fit(val=...): {epoch: evaluate's summary without "curves"}
         self.set_lr(lr)
         engine.refresh_weights(self.params)          # builds and uploads the refresh table
         torch.cuda.synchronize(dev)
@@ -722,8 +723,12 @@ def lr_schedule(lr, start_epoch, epochs, lr_decay_step=5, lr_decay_gamma=0.1):
     return out
 
 
+VAL_KEYS = ("entries", "frames", "calib", "result_dir")
+VAL_OPTIONAL = ("labels", "name", "empty_files", "inflight")
+
+
 def fit(trainer, roidb, frames, epochs, start_epoch=1, lr_decay_step=5, lr_decay_gamma=0.1, save_dir=None, log=print,
-        generator=None, target_size=600, max_rows=64, rgb_input=True, batch_size=1):
+        generator=None, target_size=600, max_rows=64, rgb_input=True, batch_size=1, val=None):
     """The training loop of trainval_net.py:183-258 at `batch_size` stereo pairs per step and rank (the reference's
     --bs, trainval_net.py:54-56) over Trainer.step_from_frames, two buffer sets per (frame shape) so that the copy of
     the next batch overlaps the running step.  At trainer.world == 1 every (frame shape, buffer set) replays a CUDA
@@ -740,8 +745,18 @@ def fit(trainer, roidb, frames, epochs, start_epoch=1, lr_decay_step=5, lr_decay
     steps; the numbers are copied to pinned memory behind an event and read one step late, so the steady state has no
     device-wide synchronise.  With save_dir, rank 0 saves trainer.checkpoint() after every epoch as
     stereo_rcnn_{epoch}_{last step}.pth (trainval_net.py:248-254).  To resume, on every rank:
-    trainer.load_checkpoint(ckpt), then fit(..., start_epoch=ckpt["epoch"]).  -> [total loss of every step, averaged
-    over the ranks]"""
+    trainer.load_checkpoint(ckpt), then fit(..., start_epoch=ckpt["epoch"]).
+
+    val: a validation split scored after every epoch -- a dict of evaluate's entries, frames, calib and result_dir,
+    optionally labels, name, empty_files and inflight, each as pipeline.evaluate takes it.  At the first validation
+    one StereoPipeline(trainer.state_dict(), throughput=True, precision of the trainer's engine) is built (one copy
+    of the weights to the device); after every later epoch pipe.eng.refresh_weights(trainer.params) writes the
+    trained masters into it in one launch.  After the epoch's checkpoint, evaluate runs on it at this target_size and
+    rgb_input, sharded over the trainer's ranks, into result_dir/epoch_<n>, replaying the graphs the first
+    validation captured.  Rank 0 logs its AP line; trainer.val_summaries[epoch] holds the summary without "curves"
+    on every rank.  Validation reads the masters and writes nothing the training reads: the steps, the random
+    words, the checkpoints and the return value are those of the same run without val.
+    -> [total loss of every step, averaged over the ranks]"""
     import os
     from .engine import GraphRunner
     from .parallel import average_losses
@@ -754,6 +769,13 @@ def fit(trainer, roidb, frames, epochs, start_epoch=1, lr_decay_step=5, lr_decay
             gen.set_state(trainer.sampler_state)
         else:
             gen.manual_seed(trainer.seed)
+    if val is not None:
+        missing = [k for k in VAL_KEYS if k not in val]
+        unknown = [k for k in val if k not in VAL_KEYS + VAL_OPTIONAL]
+        if missing or unknown:
+            raise ValueError("val: missing %s, unknown %s; it takes %s and optionally %s"
+                             % (missing, unknown, ", ".join(VAL_KEYS), ", ".join(VAL_OPTIONAL)))
+    val_pipe, val_slots = None, {}
     slots, runners, turn = {}, {}, {}
     stats_host = [torch.zeros(7, dtype=torch.float32).pin_memory() for _ in range(2)]
     stats_ev = [torch.cuda.Event() for _ in range(2)]
@@ -821,4 +843,19 @@ def fit(trainer, roidb, frames, epochs, start_epoch=1, lr_decay_step=5, lr_decay
             name = os.path.join(save_dir, "stereo_rcnn_%d_%d.pth" % (epoch, n - 1))
             torch.save(trainer.checkpoint(), name)
             log("save model: %s" % name)
+        if val is not None:
+            from . import pipeline
+            if val_pipe is None:
+                val_pipe = pipeline.StereoPipeline(trainer.state_dict(), dev, throughput=True,
+                                                   precision=trainer.engine.precision)
+            else:
+                val_pipe.eng.refresh_weights(trainer.params)
+            opts = {k: val[k] for k in VAL_OPTIONAL if k in val}
+            summary = pipeline.evaluate(val_pipe, val["entries"], val["frames"], val["calib"],
+                                        os.path.join(val["result_dir"], "epoch_%d" % epoch), target_size=target_size,
+                                        rgb_input=rgb_input, log=log, world=world,
+                                        dist=trainer.dist, slots=val_slots, **opts)
+            if "ap" in summary:
+                summary["ap"] = {k: v for k, v in summary["ap"].items() if k != "curves"}
+            trainer.val_summaries[epoch] = summary
     return totals
