@@ -2,7 +2,10 @@
 
 Per kernel: operands rounded to fp16 first, then compared with float64 torch (relative L2 < 2e-5), so that kernel
 defects are separated from rounding noise.  End to end: every returned gradient against torch fp32 autograd through
-oracle.model.trunk_fpn (relative L2 < 5e-3; the measured worst error per tensor is printed)."""
+oracle.model.trunk_fpn (relative L2 < 5e-3 for the FPN, 1e-1 for the trunk; the measured worst error per tensor is
+printed).  That bar is loose because fp16 flips ReLU masks; the wiring between the kernels is held to the kernel bar
+by test_gpu_trunk_backward_replay.py, which replays every layer in float64 from the engine's own recorded operands
+and masks (fp32 data gradients relative L2 < 2e-5, weight gradients element by element within the wgrad bound)."""
 import os
 
 import numpy as np
