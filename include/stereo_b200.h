@@ -426,7 +426,10 @@ int sb_box_rectify_devcalib(const float* boxes_all, const float* kpts_all, const
  * gathered[world][rec_floats].  Step counters live on the device: both calls are CUDA-graph capturable.  A peer
  * that never delivers sets *err_flag (device int) to 1 + its rank after timeout_s instead of hanging the GPU.
  * Replaces torch.distributed.all_gather / ncclAllGather on the data path; mailboxes[] is a HOST array of the
- * `world` device pointers (own allocation at index `rank`).                                                  */
+ * `world` device pointers (own allocation at index `rank`).  SB_EINVAL, before any launch, unless: 1 <= world <= 16;
+ * 0 <= rank < world; 0 <= slot < n_slots; rec_floats >= 4 and a multiple of 4; rec, gathered and every mailbox are
+ * non-null and 16-byte aligned; lag is 0 or 1; 0 <= timeout_s <= 1.8e10 (so never NaN).  Step counters are 32-bit:
+ * the wait of a slot's 2^32nd step returns without copying (at lag 1, the next step's too), see csrc/peer.cu.    */
 size_t sb_peer_mailbox_bytes(int n_slots, int world, int rec_floats);
 int sb_peer_alloc(size_t bytes, void** ptr);
 int sb_peer_free(void* ptr);

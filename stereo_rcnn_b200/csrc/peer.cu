@@ -19,6 +19,12 @@
 // put step t-1, which each issues (stream order) before copying out step t-2 -- so while a peer still reads t-2 the
 // fastest rank can have written at most t+1: four live records.  NCCL stays the control plane (rendezvous, handle
 // exchange, barriers).
+//
+// Counters are 32-bit and compared modulo 2^32 (flags as a signed distance, the early exit unsigned), so the exchange
+// runs straight through 2^31.  A slot's counter after 2^32 puts is 0 again, which is also the "nothing put yet" state:
+// the wait of that step (and, at lag 1, of the next one too) returns without copying, and the exchange continues
+// after it (2^32 is a multiple of the 4 parities).  So 2^32 - 1 steps per slot is the limit of an uninterrupted
+// exchange: about 80 days of one slot at 600 steps/s.
 #include "common.cuh"
 
 namespace {
@@ -90,7 +96,7 @@ peer_wait_kernel(float* __restrict__ mailbox, Layout L, int slot, int lag, float
     __shared__ unsigned s_seq;
     __shared__ int s_ok;
     const unsigned cur = ctl[L.seq_off(slot)];          // written by this rank's put (stream order)
-    if ((int)cur - lag < 1) return;                     // nothing that old has been put yet (first `lag` calls): CTA-uniform
+    if (cur < 1u + (unsigned)lag) return;               // nothing that old has been put yet (first `lag` calls): CTA-uniform
     if (threadIdx.x == 0) {
         const unsigned seq = cur - (unsigned)lag;
         const unsigned long long t0 = gtime_ns();
@@ -116,6 +122,11 @@ Layout make_layout(int n_slots, int world, int rec_floats) {
     L.n_slots = n_slots; L.world = world; L.rec_floats = rec_floats;
     return L;
 }
+
+bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
+
+// the longest wait whose nanosecond count still fits the kernel's u64
+constexpr double kMaxTimeoutS = 1.8e10;
 
 }  // namespace
 
@@ -153,8 +164,10 @@ extern "C" int sb_ipc_close(void* ptr) { return (int)cudaIpcCloseMemHandle(ptr);
 extern "C" int sb_peer_put_record(const float* rec, void* const* mailboxes, int n_slots, int world, int rec_floats,
                                   int rank, int slot, sb_stream_t stream) {
     if (!rec || !mailboxes || world < 1 || world > kMaxPeers || rank < 0 || rank >= world || slot < 0 || slot >= n_slots ||
-        rec_floats < 4 || (rec_floats & 3) || (reinterpret_cast<uintptr_t>(rec) & 15))
+        rec_floats < 4 || (rec_floats & 3) || misaligned16(rec))
         return SB_EINVAL;
+    for (int i = 0; i < world; ++i)
+        if (!mailboxes[i] || misaligned16(mailboxes[i])) return SB_EINVAL;
     PeerPtrs pp;
     for (int i = 0; i < kMaxPeers; ++i) pp.p[i] = i < world ? static_cast<float*>(mailboxes[i]) : nullptr;
     peer_put_kernel<<<world, 256, 0, sb_cs(stream)>>>(rec, pp, make_layout(n_slots, world, rec_floats), rank, slot);
@@ -166,7 +179,8 @@ extern "C" int sb_peer_put_record(const float* rec, void* const* mailboxes, int 
 extern "C" int sb_peer_wait_records(void* mailbox, int n_slots, int world, int rec_floats, int slot, int lag,
                                     float* gathered, int* err_flag, double timeout_s, sb_stream_t stream) {
     if (!mailbox || !gathered || !err_flag || world < 1 || world > kMaxPeers || slot < 0 || slot >= n_slots || lag < 0 || lag > 1 ||
-        rec_floats < 4 || (rec_floats & 3) || (reinterpret_cast<uintptr_t>(gathered) & 15))
+        rec_floats < 4 || (rec_floats & 3) || misaligned16(mailbox) || misaligned16(gathered) ||
+        !(timeout_s >= 0.0 && timeout_s <= kMaxTimeoutS))                 // also refuses NaN
         return SB_EINVAL;
     peer_wait_kernel<<<world, 128, 0, sb_cs(stream)>>>(static_cast<float*>(mailbox), make_layout(n_slots, world, rec_floats),
                                                        slot, lag, gathered, err_flag,

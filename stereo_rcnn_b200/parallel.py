@@ -50,6 +50,7 @@ class RecordGather(object):
         sequence flag (csrc/peer.cu; CUDA IPC handles travel once through torch.distributed); optionally pipelined
         (lag 1).  No NCCL kernel on the data path.  Verified bit-exact on 2 / 4 / 8 GPUs, but measured 2-3 % behind the
         per-slot NCCL communicators on the bench (N = 2: 596 vs 613 pairs/s, N = 8: 2321 vs 2388), so it is opt-in.
+        When R * C is not a multiple of 4, the result is a row-strided view of a [world, R * C rounded up to 4] buffer.
     On CPU tensors (gloo host tests) the collective is always torch.distributed's.
     world == 1: identity.  `describe()` says which path is live; a peer set-up failure is reported there, not hidden.
     """
@@ -69,8 +70,6 @@ class RecordGather(object):
         mode = mode or os.environ.get("SB_GATHER", "nccl")
         self.mode = "none" if world == 1 else ("nccl" if self.device.type != "cuda" else mode)
         self.note = ""
-        self.out = [torch.empty((world,) + self.rec_shape, dtype=torch.float32, device=self.device)
-                    for _ in range(n_slots)] if world > 1 else None
         if self.mode == "peer":
             try:
                 self._setup_peer()
@@ -82,8 +81,17 @@ class RecordGather(object):
             dist.all_reduce(ok, op=dist.ReduceOp.MIN)
             if int(ok[0]) == 0 and self.mode == "peer":
                 self.mode, self.note = "nccl", "a peer rank could not map the mailboxes, using nccl"
-        if self.mode != "peer":
+        if self.mode == "peer":
+            # the wait copies every rank's whole padded record (rec_floats floats, a float4 multiple) at a rec_floats
+            # stride, so a slot's output is a [world, rec_floats] buffer seen as [world, R, C]
+            n = self.rec_shape[0] * self.rec_shape[1]
+            self._gathered = [torch.empty(world, self.rec_floats, dtype=torch.float32, device=self.device)
+                              for _ in range(n_slots)]
+            self.out = [g[:, :n].view((world,) + self.rec_shape) for g in self._gathered]
+        else:
             self.lag = 0
+            self.out = [torch.empty((world,) + self.rec_shape, dtype=torch.float32, device=self.device)
+                        for _ in range(n_slots)] if world > 1 else None
         if self.mode == "nccl":
             self.groups = [dist.new_group() if self.device.type == "cuda" else None for _ in range(n_slots)]
 
@@ -141,7 +149,8 @@ class RecordGather(object):
             lib.check(L.sb_peer_put_record(lib.ptr(src), self._boxes, self.n_slots, self.world, self.rec_floats,
                                            self.rank, slot, st), "sb_peer_put_record")
             lib.check(L.sb_peer_wait_records(self._own, self.n_slots, self.world, self.rec_floats, slot, self.lag,
-                                             lib.ptr(out), lib.ptr(self._err), float(self.timeout_s), st),
+                                             lib.ptr(self._gathered[slot]), lib.ptr(self._err), float(self.timeout_s),
+                                             st),
                       "sb_peer_wait_records")
             return out
         self.dist.all_gather_into_tensor(out.view((-1,) + self.rec_shape[1:]), rec.contiguous(),
@@ -154,11 +163,11 @@ class RecordGather(object):
             return None if self.out is None else self.out[slot]
         from . import lib
         L = lib.load()
-        out = self.out[slot]
-        lib.check(L.sb_peer_wait_records(self._own, self.n_slots, self.world, self.rec_floats, slot, 0, lib.ptr(out),
-                                         lib.ptr(self._err), float(self.timeout_s), lib.stream_ptr()),
+        lib.check(L.sb_peer_wait_records(self._own, self.n_slots, self.world, self.rec_floats, slot, 0,
+                                         lib.ptr(self._gathered[slot]), lib.ptr(self._err), float(self.timeout_s),
+                                         lib.stream_ptr()),
                   "sb_peer_wait_records")
-        return out
+        return self.out[slot]
 
     def describe(self):
         if self.world == 1:
