@@ -310,11 +310,13 @@ int sb_permute3(const float* src, int d0, int d1, int d2, long long s0, long lon
  * per CTA and 304 CTA slots per launch, into a caller-owned device buffer of sb_conv_trace_bytes(max_launches)
  * bytes.  buf = NULL switches tracing off.  sb_conv_trace_info(id) gives launch id's {Cin, Cout, kh, M, BLOCK_N, tiles,
  * K-steps, residual, upsample, variant, max_ctas, N}, variant = 1 (fp16 operands) | 2 (data gradient) | 4 (mask).
- * No counterpart in the reference. */
+ * sb_conv_trace_epilogue(id) is 1 when launch id stored its outputs by TMA through the per-warpgroup rings, 0 when it
+ * ran the register epilogue.  No counterpart in the reference. */
 size_t sb_conv_trace_bytes(int max_launches);
 int sb_conv_trace(void* buf, int max_launches);
 int sb_conv_trace_count(void);
 int sb_conv_trace_info(int id, int* out12);
+int sb_conv_trace_epilogue(int id);
 
 /* stem: NCHW image -> conv7x7/2 + frozen BN + ReLU -> NHWC (resnet.py:111-113) */
 int sb_stem_conv(const float* im_nchw, int N, int H, int W, const float* wgt /*[64][7][7][3]*/,

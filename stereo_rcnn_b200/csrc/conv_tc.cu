@@ -24,7 +24,7 @@
 //     the TMA producer.  One mbarrier ring (full / empty) of stages sized so that nearly all shared memory holds
 //     operands (4 stages of 48 KB for 256-wide tiles, 6 of 32 KB for 128-wide ones); the producer runs ahead into
 //     the next tile while the consumers finish the epilogue of the current one.
-//   * ping-pong schedule (fp16 operands, register epilogue, tiles of at most 128 columns -- 64 with the upsample-add
+//   * ping-pong schedule (fp16 operands, no residual, tiles of at most 128 columns -- 64 with the upsample-add or an fp32 TMA box
 //     -- and a launch where some CTA gets a second tile): the CTA's j-th tile belongs to warpgroup j & 1, which
 //     issues two m64nNk16 wgmma per k16 (one per 64-row half of the A stage) and owns all 128 rows' accumulators.  The mainloops take turns (a pair of
 //     mbarriers: a warpgroup starts a tile once the other has issued its previous tile's last K-step), so each
@@ -48,6 +48,11 @@
 //     columns past Cout, a warpgroup without rows in the last tile).  Shared memory of a 128-wide residual tile: 4
 //     operand stages of 32 KB + 2 warpgroups x 4 slots x 12 KB = 96 KB of rings (64-wide: 6 x 24 KB + 2 x 3 x 12 KB;
 //     32-wide: 7 x 20 KB + 2 x 3 x 12 KB).  The TF32 mode and the data-gradient variants keep the register epilogue.
+//   * plain outputs by TMA (fp16 operands, forward, no residual or upsample-add, flat output rows that a 2-D [ld, M]
+//     map expresses): the same per-warpgroup rings without the residual producers -- the consumers take a slot once
+//     the stores of its previous entry have read it.  Slots hold both boxes when the conv writes fp32 (kEpiTma) and
+//     the fp16 box alone otherwise (kEpiTma16, 4 KB: 4 slots per warpgroup beside the register variants' stages).  A
+//     ping-pong warpgroup streams its 128 rows as two 64-row entries per chunk.
 //   * programmatic dependent launch: the prologue (barrier init, descriptor prefetch) overlaps the previous
 //     kernel's tail; dependents are released after the CTA's last operand loads are issued.
 //   * optional per-CTA phase trace (sb_conv_trace) for tools/conv_trace.py: timestamps, the schedule and the tiles
@@ -104,52 +109,64 @@ constexpr int kTraceSched = 7, kTraceTiles = 14;
 // slots, each one 32-column chunk of the warpgroup's 64 tile rows: an fp32 box [64 rows][32 columns] (residual in,
 // fp32 result out, in place; 128-byte rows, 128-byte swizzle) and an fp16 box [64 rows][32 columns] (the twin; 64-byte
 // rows, 64-byte swizzle).  Warps 9 and 10 are the residual producers of warpgroups 0 and 1.
+// The plain TMA epilogue (fp16-operand forward without a residual, flat output rows) uses the same rings without the
+// residual producers: the consumers own the slots.  Its slots hold both boxes when the conv writes an fp32 output
+// (kEpiTma) and the fp16 box alone when it writes the twin only (kEpiTma16: 4 KB slots, so 4 per warpgroup fit beside
+// the register-epilogue instantiations' operand stages).
 constexpr uint32_t kEpiBox = 64 * 128, kTwinBox = 64 * 64, kSlotBytes = kEpiBox + kTwinBox;
+enum : int { kEpiRegs = 0, kEpiTma = 1, kEpiTma16 = 2 };
 constexpr int kResProducerWarps = 2;
 constexpr int kResThreads = kThreads + 32 * kResProducerWarps;
-constexpr bool tma_epilogue(bool has_res, bool in16, bool mask) { return has_res && in16 && !mask; }
-constexpr int epi_slots(int block_n) { return block_n == 128 ? 4 : 3; }
-constexpr int conv_threads(bool stem, bool tma_epi) { return stem ? kStemThreads : tma_epi ? kResThreads : kThreads; }
-// instantiations that have a ping-pong twin: fp16 operands, the epilogue runs from registers, and a warpgroup's
-// 128 x BLOCK_N accumulators and its four rows' epilogue state fit the register budget without spills -- 168 per
-// thread at 288 threads and one CTA per SM (nine warps on four 16K-register SM sub-partitions).  At 128 columns the
-// upsample-add epilogue does not (2.4 KB of spill stores), so that one stays cooperative.
-constexpr bool pingpong_ok(int block_n, bool has_res, bool has_up, bool in16, bool stem, bool mask) {
-    return in16 && !tma_epilogue(has_res, in16, mask) && !stem && !mask && block_n <= (has_up ? 64 : 128);
+constexpr uint32_t epi_slot_bytes(int epi) { return epi == kEpiTma16 ? kTwinBox : kSlotBytes; }
+constexpr int epi_slots(int block_n, int epi) { return epi == kEpiRegs ? 0 : (epi == kEpiTma16 || block_n == 128) ? 4 : 3; }
+constexpr bool res_ring(bool has_res, int epi) { return has_res && epi != kEpiRegs; }    // residual producer warps
+constexpr int conv_threads(bool stem, bool res_producers) { return stem ? kStemThreads : res_producers ? kResThreads : kThreads; }
+// instantiations that have a ping-pong twin: fp16 operands, no residual (its ring has one producer per 64-row
+// warpgroup half), and a warpgroup's 128 x BLOCK_N accumulators and its epilogue state fit the register budget without
+// spills -- 168 per thread at 288 threads and one CTA per SM (nine warps on four 16K-register SM sub-partitions).  At
+// 128 columns the upsample-add epilogue does not (2.4 KB of spill stores), nor does the TMA epilogue with an fp32 box
+// (4-24 bytes, however its ring counters are kept), so those stay cooperative.
+constexpr bool pingpong_ok(int block_n, bool has_res, bool has_up, bool in16, bool stem, bool mask, int epi) {
+    return in16 && !has_res && !stem && !mask && block_n <= (has_up || epi == kEpiTma ? 64 : 128);
 }
 
 // operand stages, then (slots > 0) both warpgroups' epilogue rings, the 1024-byte alignment pad and the mbarriers
 // (operand ring, epilogue rings, the residual producers' start, the two ping-pong turns)
-constexpr size_t conv_smem(int block_n, int stages, int slots) {
-    return (size_t)stages * (BLOCK_M * kRowBytes + block_n * kRowBytes) + (size_t)2 * slots * kSlotBytes + 1024 +
+constexpr size_t conv_smem(int block_n, int stages, int slots, uint32_t slot_bytes) {
+    return (size_t)stages * (BLOCK_M * kRowBytes + block_n * kRowBytes) + (size_t)2 * slots * slot_bytes + 1024 +
            (2 * stages + 4 * slots + 3) * 8;
 }
 
+// EPI: kEpiRegs (epilogue from registers), kEpiTma or kEpiTma16 (through the per-warpgroup rings, stored by TMA)
 template <int BLOCK_N, int kStages, bool HAS_RES, bool HAS_UP, bool IN16, bool STEM = false, bool MASK = false,
-          bool PP = false>
-__global__ void __launch_bounds__(conv_threads(STEM, tma_epilogue(HAS_RES, IN16, MASK)), 1)
+          bool PP = false, int EPI = kEpiRegs>
+__global__ void __launch_bounds__(conv_threads(STEM, res_ring(HAS_RES, EPI)), 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                const __grid_constant__ CUtensorMap map_r, const __grid_constant__ CUtensorMap map_o,
                const __grid_constant__ CUtensorMap map_o16, const TcParams p) {
     static_assert(!STEM || (IN16 && !HAS_RES && !HAS_UP), "stem variant");
     static_assert(!MASK || (IN16 && !HAS_UP && !STEM), "mask variant");
-    static_assert(!PP || pingpong_ok(BLOCK_N, HAS_RES, HAS_UP, IN16, STEM, MASK), "ping-pong variant");
-    constexpr bool kTmaEpi = tma_epilogue(HAS_RES, IN16, MASK);
-    static_assert(!kTmaEpi || BLOCK_N <= 128, "residual layers use tiles of at most 128 columns");
+    static_assert(!PP || pingpong_ok(BLOCK_N, HAS_RES, HAS_UP, IN16, STEM, MASK, EPI), "ping-pong variant");
+    static_assert(EPI == kEpiRegs || (IN16 && !STEM && !MASK && !HAS_UP), "TMA epilogue: fp16-operand forward");
+    static_assert(!HAS_RES || !IN16 || MASK || EPI == kEpiTma, "the fp16 forward residual runs through the ring");
+    constexpr bool kTmaEpi = EPI != kEpiRegs;
+    constexpr bool kResRing = res_ring(HAS_RES, EPI);
+    static_assert(!kResRing || BLOCK_N <= 128, "residual layers use tiles of at most 128 columns");
     constexpr uint32_t kABytes = BLOCK_M * kRowBytes, kBBytes = BLOCK_N * kRowBytes;
     constexpr int BLOCK_K = IN16 ? 64 : 32;     // elements per K-step
     constexpr uint32_t kStageBytes = kABytes + kBBytes;
-    constexpr int kSlots = kTmaEpi ? epi_slots(BLOCK_N) : 0;     // epilogue ring slots per consumer warpgroup
-    constexpr int kChunks = BLOCK_N / 32;                        // ring entries per tile and warpgroup
-    // a chunk's slot is released while the next chunk is processed, so the producer needs a second slot to load it
+    constexpr int kSlots = epi_slots(BLOCK_N, EPI);              // epilogue ring slots per consumer warpgroup
+    constexpr uint32_t kSlotB = epi_slot_bytes(EPI), kTwinOff = EPI == kEpiTma16 ? 0 : kEpiBox;
+    constexpr int kChunks = BLOCK_N / 32;                        // 32-column chunks per tile
+    // a chunk's slot is released while the next chunk is processed, so a second slot must be free to fill
     static_assert(!kTmaEpi || kSlots >= 2, "epilogue ring of at least two slots");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t* epi = smem + kStages * kStageBytes;                  // [2 warpgroups][kSlots][kSlotBytes]
-    uint64_t* full = reinterpret_cast<uint64_t*>(epi + 2 * kSlots * kSlotBytes);
+    uint8_t* epi = smem + kStages * kStageBytes;                  // [2 warpgroups][kSlots][kSlotB]
+    uint64_t* full = reinterpret_cast<uint64_t*>(epi + 2 * kSlots * kSlotB);
     uint64_t* empty = full + kStages;
     uint64_t* slot_full = empty + kStages;         // [2][kSlots]: the chunk's residual box has landed
-    uint64_t* slot_empty = slot_full + 2 * kSlots; // [2][kSlots]: the chunk's output stores have read the slot
+    uint64_t* slot_empty = slot_full + 2 * kSlots; // [2][kSlots]: the output stores of the slot's last chunk have read it
     uint64_t* res_go = slot_empty + 2 * kSlots;    // the first tile's first operand loads are issued
     uint64_t* turn = res_go + 1;                   // [2] (PP): warpgroup g may start its next tile's K loop
 
@@ -166,7 +183,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     if (warp == kProducerWarp && lane == 0) {
         if (!STEM) prefetch_tmap(&map_a);
         prefetch_tmap(&map_b);
-        if (kTmaEpi) prefetch_tmap(&map_r);
+        if (kResRing) prefetch_tmap(&map_r);
         // STEM: a stage is full when the weight tile has landed (1 expect_tx arrival) and the gather threads have
         // written their patch rows.  A stage is empty when the MMAs on it of every consumer warp that reads it
         // (all eight; PP: the four of the tile's warpgroup) have completed.
@@ -182,7 +199,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             mbar_init(&slot_full[i], 1);         // the residual producer's expect_tx arrival
             mbar_init(&slot_empty[i], 1);        // the warpgroup's store thread
         }
-        if (kTmaEpi) mbar_init(res_go, 1);
+        if (kResRing) mbar_init(res_go, 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -238,7 +255,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                     // the residual producers start once the first tile's first min(K-steps, stages) operand loads
                     // are issued: with the residual loads issued alongside, the first operand stage landed ~10 k
                     // cycles after griddepcontrol.wait instead of ~3 k (H100, layers 1-4 conv3)
-                    if (kTmaEpi && tile == (int)blockIdx.x && kb == min(p.num_k_blocks, kStages) - 1) mbar_arrive(res_go);
+                    if (kResRing && tile == (int)blockIdx.x && kb == min(p.num_k_blocks, kStages) - 1) mbar_arrive(res_go);
                 }
             }
             // release the dependent launch once this CTA's last operand loads are issued: an earlier release lets the
@@ -246,7 +263,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
             if (tr) { tr[3] = gtimer(); tr[11] = clock64(); }
         }
-    } else if (kTmaEpi && warp > kProducerWarp) {
+    } else if (kResRing && warp > kProducerWarp) {
         // ===================== residual producer of warpgroup g (warps 9, 10) =====================
         // Loads the warpgroup's residual chunks in (tile, chunk) order into its ring as soon as a slot is empty, so
         // the next tile's chunks stream in under this tile's last chunks and the next main loop.  Every chunk of
@@ -263,7 +280,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                     uint64_t* bar = &slot_full[g * kSlots + slot];
                     mbar_wait(&slot_empty[g * kSlots + slot], sphase ^ 1);
                     mbar_expect_tx(bar, kEpiBox);
-                    tma_load_2d(&map_r, bar, epi + (g * kSlots + slot) * kSlotBytes, nt * BLOCK_N + 32 * c,
+                    tma_load_2d(&map_r, bar, epi + (g * kSlots + slot) * kSlotB, nt * BLOCK_N + 32 * c,
                                 mt * BLOCK_M + 64 * g);
                     if (++slot == kSlots) { slot = 0; sphase ^= 1; }
                 }
@@ -433,18 +450,24 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             if (lane == 0) mbar_arrive(&empty[prev]);
 
             if constexpr (kTmaEpi) {
-                // ---- residual epilogue through the warpgroup's ring, one 32-column chunk at a time.  The residual
-                // producer has loaded the chunk's 64 residual rows into the slot's fp32 box; every thread adds its
-                // accumulator pairs to them in place and writes the fp16 twin beside them, then one thread stores
-                // both boxes by TMA (rows past M and columns past Cout are clipped) as one bulk group.  The slot of
-                // the chunk before is handed back once its group has read it, so the warpgroup goes straight on to
-                // the next chunk and the global writes drain under the next chunks and the next tile's MMAs.
-                const int rl = 16 * (warp & 3) + (lane >> 2);     // rows rl and rl + 8 of the warpgroup's 64
-                const int row0 = mt * BLOCK_M + 64 * wg;
+                // ---- TMA epilogue through the warpgroup's ring, one box of 64 rows x 32 columns per ring entry: a
+                // cooperative warpgroup streams its 64 rows chunk by chunk, a ping-pong warpgroup all 128 rows as two
+                // 64-row entries per chunk (the slots, tensor maps and ring accounting stay those of the 64-row
+                // residual ring).  With a residual, its producer has loaded the entry's residual rows into the slot's
+                // fp32 box and every thread adds its accumulator pairs to them in place; without, the slot is taken
+                // once the stores of its previous entry have read it.  Every thread writes its values (and the fp16
+                // twin) into the slot, then one thread stores the boxes by TMA (rows past M and columns past Cout
+                // are clipped) as one bulk group.  The slot of the entry before is handed back once its group has
+                // read it, so the warpgroup goes straight on to the next entry and the global writes drain under the
+                // next entries and the next tile's MMAs.
+                const int rl = 16 * (warp & 3) + (lane >> 2);     // rows rl and rl + 8 of the entry's 64
 #pragma unroll
-                for (int ch = 0; ch < kChunks; ++ch) {
-                    const uint32_t rbuf = smem_u32(epi) + (wg * kSlots + slot) * kSlotBytes, tbuf = rbuf + kEpiBox;
-                    mbar_wait(&slot_full[wg * kSlots + slot], sphase);
+                for (int e = 0; e < kChunks * kHalves; ++e) {
+                    const int ch = e / kHalves, hf = e % kHalves;
+                    const int row0 = mt * BLOCK_M + 64 * (PP ? hf : wg);
+                    const uint32_t rbuf = smem_u32(epi) + (wg * kSlots + slot) * kSlotB, tbuf = rbuf + kTwinOff;
+                    if (kResRing) mbar_wait(&slot_full[wg * kSlots + slot], sphase);
+                    else mbar_wait(&slot_empty[wg * kSlots + slot], sphase ^ 1);
 #pragma unroll
                     for (int jj = 0; jj < 4; ++jj) {
                         const int j = 4 * ch + jj;
@@ -457,15 +480,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                         for (int h = 0; h < 2; ++h) {
                             const uint32_t row = (uint32_t)(rl + 8 * h);
                             const uint32_t ra = rbuf + swz128(row * 128 + (cl & 31) * 4);
-                            float2 r = lds64f(ra);
-                            float x0 = fmaf(acc[4 * j + 2 * h], sc.x, sh.x);
-                            float x1 = fmaf(acc[4 * j + 2 * h + 1], sc.y, sh.y);
-                            if (res_biased) { r.x = sb_unbias_tf32(r.x); r.y = sb_unbias_tf32(r.y); }
-                            x0 += r.x; x1 += r.y;
+                            const int ai = hf * kAcc + 4 * j + 2 * h;
+                            float x0 = fmaf(acc[ai], sc.x, sh.x);
+                            float x1 = fmaf(acc[ai + 1], sc.y, sh.y);
+                            if (kResRing) {
+                                float2 r = lds64f(ra);
+                                if (res_biased) { r.x = sb_unbias_tf32(r.x); r.y = sb_unbias_tf32(r.y); }
+                                x0 += r.x; x1 += r.y;
+                            }
                             if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
                             if (out_mode == 1) { x0 = sb_round_tf32(x0); x1 = sb_round_tf32(x1); }
                             else if (out_mode == 2) { x0 = sb_bias_tf32(x0); x1 = sb_bias_tf32(x1); }
-                            sts64f(ra, x0, x1);
+                            if (EPI == kEpiTma) sts64f(ra, x0, x1);
                             if (d.out16) {   // fp16 twin (round to nearest) for the next tensor-core consumer
                                 if (out_mode == 2) { x0 = sb_unbias_tf32(x0); x1 = sb_unbias_tf32(x1); }
                                 const __half2 hv = __floats2half2_rn(x0, x1);
@@ -478,12 +504,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                     if (store_thread) {
                         const int col = nt * BLOCK_N + 32 * ch;
                         if (row0 < p.M && col < d.Cout) {
-                            if (d.out) tma_store_2d(&map_o, rbuf, col, row0);
+                            if (EPI == kEpiTma && d.out) tma_store_2d(&map_o, rbuf, col, row0);
                             if (d.out16) tma_store_2d(&map_o16, tbuf, col, row0);
                         }
-                        bulk_commit();                    // one group per chunk, empty or not
-                        if (ch > 0) {
-                            bulk_wait_read<1>();          // all groups but this chunk's have read their slots
+                        bulk_commit();                    // one group per entry, empty or not
+                        if (e > 0) {
+                            bulk_wait_read<1>();          // all groups but this entry's have read their slots
                             mbar_arrive(&slot_empty[wg * kSlots + held]);
                         }
                     }
@@ -691,19 +717,19 @@ struct TcMaps {
 // PP: the ping-pong schedule.  An instantiation that has a ping-pong twin runs it when some CTA gets a second tile.
 // With one tile per CTA there is no other tile's epilogue to hide, and a warpgroup alone would run all 128 rows'.
 
-template <int BN, int ST, bool RES, bool UP, bool IN16, bool STEM = false, bool MASK = false, bool PP = false>
+template <int BN, int ST, bool RES, bool UP, bool IN16, bool STEM = false, bool MASK = false, bool PP = false,
+          int EPI = kEpiRegs>
 int launch_t(const TcMaps& m, const TcParams& p, cudaStream_t st) {
     const int tiles = p.num_m_tiles * p.num_n_tiles;
     int slots = sb_num_sms();
     if (p.d.max_ctas > 0 && p.d.max_ctas < slots) slots = p.d.max_ctas;
     const int grid = tiles < slots ? tiles : slots;
-    if constexpr (!PP && pingpong_ok(BN, RES, UP, IN16, STEM, MASK)) {
-        if (tiles > grid) return launch_t<BN, ST, RES, UP, IN16, STEM, MASK, true>(m, p, st);
+    if constexpr (!PP && pingpong_ok(BN, RES, UP, IN16, STEM, MASK, EPI)) {
+        if (tiles > grid) return launch_t<BN, ST, RES, UP, IN16, STEM, MASK, true, EPI>(m, p, st);
     }
-    constexpr bool tma_epi = tma_epilogue(RES, IN16, MASK);
-    constexpr size_t smem = conv_smem(BN, ST, tma_epi ? epi_slots(BN) : 0);
+    constexpr size_t smem = conv_smem(BN, ST, epi_slots(BN, EPI), epi_slot_bytes(EPI));
     static_assert(smem <= 227 * 1024, "smem budget");
-    auto kern = conv_tc_kernel<BN, ST, RES, UP, IN16, STEM, MASK, PP>;
+    auto kern = conv_tc_kernel<BN, ST, RES, UP, IN16, STEM, MASK, PP, EPI>;
     static bool attr_done[kSbMaxDevices] = {false};
     bool& attr = attr_done[sb_cur_device()];
     if (!attr) {
@@ -713,7 +739,7 @@ int launch_t(const TcMaps& m, const TcParams& p, cudaStream_t st) {
     }
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(conv_threads(STEM, tma_epi));
+    cfg.blockDim = dim3(conv_threads(STEM, res_ring(RES, EPI)));
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
     cudaLaunchAttribute attrs[1];
@@ -728,9 +754,10 @@ int launch_t(const TcMaps& m, const TcParams& p, cudaStream_t st) {
     return SB_OK;
 }
 
-// ST: operand stages; ST_RES: operand stages beside the TMA residual epilogue's rings (0: no such variant)
-template <int BN, int ST, int ST_RES>
-int launch(const TcMaps& m, const TcParams& p, bool dgrad, cudaStream_t st) {
+// ST: operand stages beside no ring or 4 KB slots (kEpiTma16); ST_EPI: operand stages beside the 12 KB slots of
+// kEpiTma (the residual, fp32 outputs)
+template <int BN, int ST, int ST_EPI>
+int launch(const TcMaps& m, const TcParams& p, bool dgrad, int epi, cudaStream_t st) {
     const bool res = p.d.residual != nullptr, up = p.d.up_src != nullptr;   // never both (supported())
     if (dgrad && (p.mask16 || res))     // fp16 operands, never an upsample source (sb_conv2d_tc_dgrad)
         return res ? launch_t<BN, ST, true, false, true, false, true>(m, p, st)
@@ -738,16 +765,18 @@ int launch(const TcMaps& m, const TcParams& p, bool dgrad, cudaStream_t st) {
     if (p.d.in_dtype == 1) {
         if (up) return launch_t<BN, ST, false, true, true>(m, p, st);
         if (res) {
-            if constexpr (ST_RES > 0) return launch_t<BN, ST_RES, true, false, true>(m, p, st);
+            if constexpr (BN <= 128) return launch_t<BN, ST_EPI, true, false, true, false, false, false, kEpiTma>(m, p, st);
             return SB_EINVAL;
         }
+        if (epi == kEpiTma) return launch_t<BN, ST_EPI, false, false, true, false, false, false, kEpiTma>(m, p, st);
+        if (epi == kEpiTma16) return launch_t<BN, ST, false, false, true, false, false, false, kEpiTma16>(m, p, st);
         return launch_t<BN, ST, false, false, true>(m, p, st);
     }
     if (up) return launch_t<BN, ST, false, true, false>(m, p, st);
     return res ? launch_t<BN, ST, true, false, false>(m, p, st) : launch_t<BN, ST, false, false, false>(m, p, st);
 }
 
-// The fp16-operand forward residual epilogue moves the residual and both outputs as 2-D [ld, M] TMA boxes: output
+// The fp16-operand forward TMA epilogue moves the residual and both outputs as 2-D [ld, M] TMA boxes: output
 // pixels must be contiguous rows (m * out_w_stride), and row strides and bases 16-byte aligned.  The twin's rows must
 // also be a whole number of 16-byte units (Cout % 8 == 0): with Cout = 36 or 100 the bulk tensor store was measured
 // to write fp16 columns past Cout, into the neighbouring channels of a wider row (H100, CUDA 12.9).
@@ -798,6 +827,7 @@ unsigned long long* g_trace = nullptr;
 int g_trace_cap = 0, g_trace_n = 0;
 struct TraceInfo { int v[12]; };
 TraceInfo g_trace_info[4096];
+int g_trace_epi[4096];
 }  // namespace
 
 extern "C" size_t sb_conv_trace_bytes(int max_launches) {
@@ -816,6 +846,7 @@ extern "C" int sb_conv_trace_info(int id, int* out12) {
     return SB_OK;
 }
 extern "C" int sb_conv_trace_count(void) { return g_trace_n; }
+extern "C" int sb_conv_trace_epilogue(int id) { return id < 0 || id >= g_trace_n ? SB_EINVAL : g_trace_epi[id]; }
 
 namespace {
 // rows: flat 128-pixel tiles loaded by TMA im2col for a 3x3 conv (sb_conv2d_tc_rows; the caller has checked the
@@ -848,6 +879,18 @@ int conv2d_tc(const sb_conv_desc* d, const __half* mask16, bool dgrad, bool rows
     // the operand stages
     if (d->residual && BN == 256) BN = 128;
     p.num_n_tiles = (d->Cout + BN - 1) / BN;
+    // the TMA epilogue: fp16-operand forward on flat rows (1x1, or 3x3 through the rows entry) whose outputs are 2-D
+    // [ld, M] maps.  The TF32 mode, the data gradient, the upsample-add and 8x16 patches keep the register epilogue.
+    int epi = kEpiRegs;
+    if (f16 && !dgrad && !d->up_src && !p.patch && tma_epilogue_layout_ok(d))
+        epi = d->out || d->residual ? kEpiTma : kEpiTma16;
+    if (epi == kEpiTma && !d->residual && BN == 128) {
+        // no ping-pong twin (pingpong_ok): where a CTA gets a second tile, the register epilogue's ping-pong hides
+        // the epilogue under the other warpgroup's MMAs, which a cooperative TMA epilogue cannot
+        int ctas = sb_num_sms();
+        if (d->max_ctas > 0 && d->max_ctas < ctas) ctas = d->max_ctas;
+        if ((long long)p.num_m_tiles * p.num_n_tiles > ctas) epi = kEpiRegs;
+    }
     if (g_trace && g_trace_n < g_trace_cap) {
         const int id = g_trace_n++;
         p.trace = g_trace + (size_t)id * kTraceCtas * kTraceWords;
@@ -856,6 +899,7 @@ int conv2d_tc(const sb_conv_desc* d, const __half* mask16, bool dgrad, bool rows
         v[6] = p.num_k_blocks; v[7] = d->residual ? 1 : 0; v[8] = d->up_src ? 1 : 0;
         v[9] = (f16 ? 1 : 0) | (dgrad ? 2 : 0) | (mask16 ? 4 : 0);     // operand type and entry point
         v[10] = d->max_ctas; v[11] = d->N;
+        g_trace_epi[id] = epi != kEpiRegs ? 1 : 0;
     }
     TcMaps m;
     memset(&m, 0, sizeof(m));
@@ -881,13 +925,13 @@ int conv2d_tc(const sb_conv_desc* d, const __half* mask16, bool dgrad, bool rows
         cuuint32_t box[2] = {(cuuint32_t)BLOCK_K, (cuuint32_t)BN};
         if (!make_map(&mb, d->wgt, 2, dims, strides, box, f16)) return SB_EINVAL;
     }
-    if (d->residual && f16 && !dgrad) {
-        // TMA residual epilogue: [Cout, M] boxes of 64 rows and 32 columns, one ring chunk each; the fp16 box has
-        // 64-byte rows, so it is 64-byte swizzled
+    if (epi != kEpiRegs) {
+        // TMA epilogue: [Cout, M] boxes of 64 rows and 32 columns, one ring entry each; the fp16 box has 64-byte rows,
+        // so it is 64-byte swizzled
         const cuuint64_t dims[2] = {(cuuint64_t)d->Cout, (cuuint64_t)p.M};
         const cuuint32_t box32[2] = {32, 64};
         const cuuint64_t rs[1] = {(cuuint64_t)d->res_ld * 4};
-        if (!make_map(&m.r, d->residual, 2, dims, rs, box32, false)) return SB_EINVAL;
+        if (d->residual && !make_map(&m.r, d->residual, 2, dims, rs, box32, false)) return SB_EINVAL;
         const cuuint64_t os[1] = {(cuuint64_t)d->out_w_stride * 4}, os16[1] = {(cuuint64_t)d->out_w_stride * 2};
         if (d->out && !make_map(&m.o, d->out + d->out_coff, 2, dims, os, box32, false)) return SB_EINVAL;
         if (d->out16 && !make_map(&m.o16, reinterpret_cast<const __half*>(d->out16) + d->out_coff, 2, dims, os16,
@@ -895,11 +939,11 @@ int conv2d_tc(const sb_conv_desc* d, const __half* mask16, bool dgrad, bool rows
             return SB_EINVAL;
     }
     cudaStream_t st = sb_cs(stream);
-    switch (BN) {        // <BN, operand stages, operand stages beside the residual epilogue rings>
-        case 32: return launch<32, 9, 7>(m, p, dgrad, st);
-        case 64: return launch<64, 8, 6>(m, p, dgrad, st);
-        case 256: return launch<256, 4, 0>(m, p, dgrad, st);
-        default: return launch<128, 6, 4>(m, p, dgrad, st);
+    switch (BN) {        // <BN, operand stages, operand stages beside the 12 KB-slot rings>
+        case 32: return launch<32, 9, 7>(m, p, dgrad, epi, st);
+        case 64: return launch<64, 8, 6>(m, p, dgrad, epi, st);
+        case 256: return launch<256, 4, 3>(m, p, dgrad, epi, st);
+        default: return launch<128, 6, 4>(m, p, dgrad, epi, st);
     }
 }
 }  // namespace

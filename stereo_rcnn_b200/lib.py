@@ -130,6 +130,7 @@ _SIGS = {
     "sb_conv_trace_bytes": (c_size_t, [c_int]),
     "sb_conv_trace": (c_int, [c_void_p, c_int]),
     "sb_conv_trace_count": (c_int, []),
+    "sb_conv_trace_epilogue": (c_int, [c_int]),
     "sb_conv_trace_info": (c_int, [c_int, ctypes.POINTER(c_int)]),
     "sb_stem_conv": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "sb_stem_im2col": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),

@@ -3,7 +3,8 @@
 ncu serialises kernels and flushes caches, so it cannot show how the launches of a CUDA-graph replay overlap
 (PDL prologues, the left/right chains on two streams).  The conv kernel can stamp %globaltimer / clock64 per
 CTA at: entry, after griddepcontrol.wait, first operand stage landed, last MMA issued, first tile's epilogue
-done, CTA exit, and which schedule the CTA's two consumer warpgroups ran (cooperative or ping-pong).  This tool
+done, CTA exit, and which schedule the CTA's two consumer warpgroups ran (cooperative or ping-pong); the host
+records which epilogue each launch ran (from registers, or stored by TMA through the per-warpgroup rings).  This tool
 captures the forward into a graph with tracing on, replays it, and prints per launch: start / end relative to the
 step, the span, and the median per-CTA phase durations.
 
@@ -55,11 +56,12 @@ def main():
     assert L.sb_conv_trace(buf.data_ptr(), a.max_launches) == 0
     r = engine.GraphRunner(fwd, [], warmup=0)
     n = L.sb_conv_trace_count()
-    infos = []
+    infos, epis = [], []
     for i in range(n):
         v = (ctypes.c_int * 12)()
         L.sb_conv_trace_info(i, v)
         infos.append(list(v))
+        epis.append(L.sb_conv_trace_epilogue(i))
     L.sb_conv_trace(None, 0)
     flush = torch.empty(64 * 1024 * 1024, dtype=torch.float32, device="cuda")
     for _ in range(3):
@@ -94,15 +96,16 @@ def main():
             fill_cyc=float(np.median(k2 - k1)), mma_cyc=float(np.median(k3 - k2)),
             epi1_cyc=float(np.median(k4 - k2)), tail_cyc=float(np.median(k5 - k3)),
             cta_cyc=float(np.median(k5 - k1)), cta_cyc_max=float((k5 - k1).max()),
-            start_skew_us=float(t1.max() - t1.min()) / 1e3, pingpong=int(c[0, 7])))
+            start_skew_us=float(t1.max() - t1.min()) / 1e3, pingpong=int(c[0, 7]),
+            epilogue="tma" if epis[i] == 1 else "reg"))
     os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
     with open(a.out, "w") as f:
         json.dump(dict(step_ms=step_ms, launches=rows), f)
     print("graph step %.3f ms, %d traced conv launches" % (step_ms, len(rows)))
-    print(" id  cin cout k      M  BN tiles ctas pp | start   work0     end |  span  wspan  wait | fill   mma  epi1  tail   cta ctamax (cycles) skew_us")
+    print(" id  cin cout k      M  BN tiles ctas pp epi | start   work0     end |  span  wspan  wait | fill   mma  epi1  tail   cta ctamax (cycles) skew_us")
     for x in rows:
-        print("%3d %4d %4d %d %6d %3d %5d %4d %2d | %6.1f %6.1f %6.1f | %5.1f %5.1f %5.1f | %5.0f %5.0f %5.0f %5.0f %6.0f %6.0f  %5.1f" % (
-            x["id"], x["cin"], x["cout"], x["k"], x["M"], x["BN"], x["tiles"], x["ctas"], x["pingpong"],
+        print("%3d %4d %4d %d %6d %3d %5d %4d %2d %3s | %6.1f %6.1f %6.1f | %5.1f %5.1f %5.1f | %5.0f %5.0f %5.0f %5.0f %6.0f %6.0f  %5.1f" % (
+            x["id"], x["cin"], x["cout"], x["k"], x["M"], x["BN"], x["tiles"], x["ctas"], x["pingpong"], x["epilogue"],
             x["start_us"], x["first_work_us"], x["end_us"], x["span_us"], x["work_span_us"], x["wait_us"],
             x["fill_cyc"], x["mma_cyc"], x["epi1_cyc"], x["tail_cyc"], x["cta_cyc"], x["cta_cyc_max"], x["start_skew_us"]))
 
