@@ -232,14 +232,27 @@ int sb_conv2d_tc_rows(const sb_conv_desc* d, sb_stream_t stream);
  * sb_fpn_grad_combine -- gradient of one FPN level: out = scale * dp + up^T(dt) + scatter2(scale * dp6) over NHWC fp32
  *   [N,H,W,C]; up^T transposes the align_corners bilinear upsample of stereo_rcnn.py:91-108 from the fine [N,TH,TW,C] dt
  *   (a gather, fixed order); dp6 [N,H6,W6,C] is the gradient of P6 = P5[::2, ::2] (stereo_rcnn.py:168).  dp, dt and dp6
- *   may each be NULL; out (fp32) and/or out16 (fp16 twin) receive the result.                                      */
+ *   may each be NULL; out (fp32) and/or out16 (fp16 twin) receive the result.
+ * The _devscale twins of these and of the backward entry points below (sb_rpn_head_grad, sb_conv_wgrad_acc,
+ *   sb_box_tail_backward, sb_kpts_tail_backward) take the gradient scale as `const float* grad_scale` (fp32 [1] in
+ *   DEVICE memory, read by the kernels; sb_fpn_grad_combine_devscale's `scale` likewise) in place of the host float:
+ *   sb_conv_wgrad*_devscale divide by *grad_scale as 1.0f / *grad_scale (the host passes inv_grad_scale; the two agree
+ *   when the scale is a power of two).  Otherwise the same kernels, operation order and argument checks as the float
+ *   entry point, plus SB_EINVAL for a NULL scale pointer; the results are bit-identical for equal values.  A captured
+ *   graph then follows a scale the device changes between replays (sb_loss_scale_update).                          */
 int sb_conv2d_tc_dgrad(const sb_conv_desc* d, const void* mask16, sb_stream_t stream);
 size_t sb_conv_wgrad_workspace(int N, int H, int W, int Cin, int Cout, int k);
 int sb_conv_wgrad(const void* dy16, const void* x16, int N, int H, int W, int Cin, int Cout, int k,
                   const float* scale, float inv_grad_scale, float* dw, const float* dy32, float* db, int* nonfinite,
                   void* workspace, size_t workspace_bytes, sb_stream_t stream);
+int sb_conv_wgrad_devscale(const void* dy16, const void* x16, int N, int H, int W, int Cin, int Cout, int k,
+                           const float* scale, const float* grad_scale, float* dw, const float* dy32, float* db,
+                           int* nonfinite, void* workspace, size_t workspace_bytes, sb_stream_t stream);
 int sb_fpn_grad_combine(const float* dp, const float* dt, int N, int H, int W, int TH, int TW, int C,
                         const float* dp6, int H6, int W6, float scale, float* out, void* out16, sb_stream_t stream);
+int sb_fpn_grad_combine_devscale(const float* dp, const float* dt, int N, int H, int W, int TH, int TW, int C,
+                                 const float* dp6, int H6, int W6, const float* scale, float* out, void* out16,
+                                 sb_stream_t stream);
 
 /* ------------------------------------------------- backward pass of the stereo RPN (fp16 operands, fp32 accumulate) ----
  * Together these replace the autograd of lib/model/rpn/stereo_rpn.py:73-95 (RPN_Conv, RPN_cls_score,
@@ -256,11 +269,18 @@ int sb_fpn_grad_combine(const float* dp, const float* dt, int N, int H, int W, i
  *   are bit-identical to sb_conv_wgrad's.  Workspace of sb_conv_wgrad_acc_workspace bytes.                        */
 int sb_rpn_head_grad(const float* d_cls_score, const float* d_bbox_pred, int B, int P, float grad_scale,
                      void* dhead16, float* dhead32, sb_stream_t stream);
+int sb_rpn_head_grad_devscale(const float* d_cls_score, const float* d_bbox_pred, int B, int P, const float* grad_scale,
+                              void* dhead16, float* dhead32, sb_stream_t stream);
 size_t sb_conv_wgrad_acc_workspace(int N, int H, int W, int Cin, int Cout, int k);
 int sb_conv_wgrad_acc(const void* dy16, int dy_ld, const void* x16, int x_ld, int N, int H, int W, int Cin, int Cout,
                       int k, const float* scale, float inv_grad_scale, const float* dy32, int dy32_ld, int accumulate,
                       int rows, int split, float* dw, float* db, float* dw_hi, float* db_hi, int* nonfinite,
                       void* workspace, size_t workspace_bytes, sb_stream_t stream);
+int sb_conv_wgrad_acc_devscale(const void* dy16, int dy_ld, const void* x16, int x_ld, int N, int H, int W, int Cin,
+                               int Cout, int k, const float* scale, const float* grad_scale, const float* dy32,
+                               int dy32_ld, int accumulate, int rows, int split, float* dw, float* db, float* dw_hi,
+                               float* db_hi, int* nonfinite, void* workspace, size_t workspace_bytes,
+                               sb_stream_t stream);
 
 /* ------------------------------------------------- backward pass of the R-CNN heads ----
  * Together with sb_conv2d_tc_dgrad / sb_conv_wgrad these replace the autograd of lib/model/stereo_rcnn/resnet.py:256-286
@@ -298,11 +318,20 @@ int sb_box_tail_backward(const float* d_cls_score, const float* d_bbox_pred, con
                          const float* w_dim, float mask_scale, float grad_scale, float* dw_cls, float* db_cls,
                          float* dw_box, float* db_box, float* dw_dim, float* db_dim, void* dz16, float* dz32,
                          int* nonfinite, sb_stream_t stream);
+int sb_box_tail_backward_devscale(const float* d_cls_score, const float* d_bbox_pred, const float* d_dim_orien_pred,
+                                  const float* fc7, int R, int K, int n_classes, const float* w_cls,
+                                  const float* w_box, const float* w_dim, float mask_scale, const float* grad_scale,
+                                  float* dw_cls, float* db_cls, float* dw_box, float* db_box, float* dw_dim,
+                                  float* db_dim, void* dz16, float* dz32, int* nonfinite, sb_stream_t stream);
 size_t sb_kpts_tail_backward_workspace(int R, int C);
 int sb_kpts_tail_backward(const void* up16, int R, int G, int C, const float* w, const float* d_kpts_pred,
                           const float* d_left_border_pred, const float* d_right_border_pred, float grad_scale,
                           void* dup16, float* dw, float* db, float* db_up, int* nonfinite, void* workspace,
                           size_t workspace_bytes, sb_stream_t stream);
+int sb_kpts_tail_backward_devscale(const void* up16, int R, int G, int C, const float* w, const float* d_kpts_pred,
+                                   const float* d_left_border_pred, const float* d_right_border_pred,
+                                   const float* grad_scale, void* dup16, float* dw, float* db, float* db_up,
+                                   int* nonfinite, void* workspace, size_t workspace_bytes, sb_stream_t stream);
 int sb_permute3(const float* src, int d0, int d1, int d2, long long s0, long long s1, long long s2, float* dst,
                 sb_stream_t stream);
 
@@ -371,6 +400,10 @@ int sb_prep_image_size(int H, int W, double scale, int* Ho, int* Wo);
 int sb_prep_image(const uint8_t* img, int H, int W, double scale, int rgb_input, float* out, sb_stream_t stream);
 /* L2 flush helper for benchmarks: writes `bytes` of scratch */
 int sb_fill(float* p, size_t n, float v, sb_stream_t stream);
+/* p[0..n) = 1.0f / *v with v fp32 [1] in device memory (exact for a power of two): the per-channel unscale vectors of
+ * the backward's data-gradient epilogues, following a loss scale that lives on the device.  SB_EINVAL for a NULL v,
+ * or a NULL p with n > 0. */
+int sb_fill_reciprocal(float* p, size_t n, const float* v, sb_stream_t stream);
 /* number of kernel launches issued by this library since load (bench "gpu_launches") */
 unsigned long long sb_launch_count(void);
 
@@ -538,6 +571,15 @@ int sb_clip_gradient(float* const* grads, const size_t* counts, int n_tensors, f
  *   torch.cuda.amp.GradScaler's skip-on-overflow.  SB_EINVAL before any launch for a null pointer, n_tensors < 1, a
  *   zero count, a negative or non-finite weight_decay / lr_mult, or a non-finite momentum.
  *
+ * sb_loss_scale_update -- torch.cuda.amp.GradScaler.update (torch._amp_update_scale_) in one thread on the device:
+ *   when *found_inf != 0, *scale *= backoff_factor and *growth_tracker = 0; otherwise *growth_tracker + 1, and when that
+ *   reaches growth_interval, *scale *= growth_factor and *growth_tracker = 0.  The scale is held within [2^-32, 2^32]:
+ *   a growth past 2^32 leaves it unchanged (and resets the tracker, as torch does for a non-finite growth), a backoff
+ *   below 2^-32 stops at 2^-32.  With power-of-two factors and a power-of-two start the scale and its reciprocal stay
+ *   exact powers of two.  scale fp32 [1], growth_tracker and found_inf int32 [1], all device memory; graph-capturable.
+ *   SB_EINVAL before any launch for a null pointer, a factor that is not a power of two, growth_factor <= 1,
+ *   backoff_factor >= 1 or growth_interval < 1.
+ *
  * sb_pack_plan / sb_pack_weights -- rewrite derived weight copies (packed, transposed, rounded, scaled) from fp32
  *   master tensors, one launch for a whole table of targets.  Target t maps a 4-d index (i0, i1, i2, i3) < shape:
  *       v = src[src_offset + sum_k i_k src_stride[k]]                    (strides may be negative: a tap flip)
@@ -579,6 +621,8 @@ typedef struct sb_pack_target {
 int sb_sgd_step(float* const* params, float* const* grads, float* const* moms, const size_t* counts,
                 const float* weight_decay, const float* lr_mult, int n_tensors, const float* lr, float momentum,
                 const int* skip, int* skipped, sb_stream_t stream);
+int sb_loss_scale_update(const int* found_inf, float* scale, int* growth_tracker, float growth_factor,
+                         float backoff_factor, int growth_interval, sb_stream_t stream);
 int sb_pack_plan(sb_pack_target* targets, int n_targets, long long* n_tiles);
 int sb_pack_weights(const sb_pack_target* targets, const sb_pack_target* targets_dev, int n_targets,
                     sb_stream_t stream);

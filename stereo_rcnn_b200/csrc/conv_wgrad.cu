@@ -186,12 +186,17 @@ __device__ __forceinline__ void store_row_value(float* lo, float* hi, int split,
     if (nonfinite && !isfinite(v)) *nonfinite = 1;
 }
 
+// DEV_SCALE: the gradient scale is read from grad_scale (device, fp32 [1]) and inv_scale = 1 / *grad_scale, exact for
+// a power of two; otherwise inv_scale is the host's
+template <bool DEV_SCALE>
 __global__ void wgrad_reduce_kernel(const float* __restrict__ part, WgParams p, int Cin, WgOut o,
-                                    const float* __restrict__ scale, float inv_scale, int* nonfinite) {
+                                    const float* __restrict__ scale, float inv_scale,
+                                    const float* __restrict__ grad_scale, int* nonfinite) {
     const int taps = p.k * p.k;
     const long long total = (long long)o.rows * Cin * taps;
     const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= total) return;
+    if (DEV_SCALE) inv_scale = 1.0f / __ldg(grad_scale);
     const int co = (int)(e / ((long long)Cin * taps));
     const int rem = (int)(e - (long long)co * Cin * taps);
     const int ci = rem / taps, tap = rem - ci * taps;
@@ -216,10 +221,12 @@ __global__ void colsum_partial_kernel(const float* __restrict__ dy, long long M,
     }
 }
 
-__global__ void colsum_final_kernel(const float* __restrict__ partial, int chunks, int C, float inv_scale, WgOut o,
-                                    int* nonfinite) {
+template <bool DEV_SCALE>
+__global__ void colsum_final_kernel(const float* __restrict__ partial, int chunks, int C, float inv_scale,
+                                    const float* __restrict__ grad_scale, WgOut o, int* nonfinite) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= o.rows) return;
+    if (DEV_SCALE) inv_scale = 1.0f / __ldg(grad_scale);
     float acc = 0.f;
     for (int i = 0; i < chunks; ++i) acc += partial[(size_t)i * C + c];
     store_row_value(o.db, o.db_hi, o.split, c, 1, 0, acc * inv_scale, o.accumulate, nonfinite);
@@ -278,10 +285,10 @@ size_t wgrad_workspace(int N, int H, int W, int Cin, int Cout, int k) {
 bool misaligned(const void* q, uintptr_t a) { return (reinterpret_cast<uintptr_t>(q) & (a - 1)) != 0; }
 
 // dy16 / x16 / dy32 rows (pixels) are dy_ld / x_ld / dy32_ld elements apart; every argument is checked before the
-// first launch
+// first launch.  grad_scale (device, may be NULL): the gradient scale read on the device in place of inv_grad_scale
 int conv_wgrad(const void* dy16, int dy_ld, const void* x16, int x_ld, int N, int H, int W, int Cin, int Cout, int k,
-               const float* scale, float inv_grad_scale, const float* dy32, int dy32_ld, WgOut o, int* nonfinite,
-               void* workspace, size_t workspace_bytes, cudaStream_t st) {
+               const float* scale, float inv_grad_scale, const float* grad_scale, const float* dy32, int dy32_ld,
+               WgOut o, int* nonfinite, void* workspace, size_t workspace_bytes, cudaStream_t st) {
     if (!dy16 || !x16 || !o.dw || N < 1 || H < 1 || W < 1 || (k != 1 && k != 3)) return SB_EINVAL;
     if (Cin < 64 || Cout < 64 || Cin % 64 || Cout % 64 || (o.db && !dy32)) return SB_EINVAL;
     if (dy_ld < Cout || x_ld < Cin || dy_ld % 8 || x_ld % 8 || (dy32 && dy32_ld < Cout)) return SB_EINVAL;
@@ -322,7 +329,12 @@ int conv_wgrad(const void* dy16, int dy_ld, const void* x16, int x_ld, int N, in
     SB_LAUNCHED();
     SB_CHECK_LAUNCH();
     const long long total = (long long)o.rows * Cin * k * k;
-    wgrad_reduce_kernel<<<sb_div_up(total, 256), 256, 0, st>>>(p.part, p, Cin, o, scale, inv_grad_scale, nonfinite);
+    if (grad_scale)
+        wgrad_reduce_kernel<true><<<sb_div_up(total, 256), 256, 0, st>>>(p.part, p, Cin, o, scale, 0.f, grad_scale,
+                                                                        nonfinite);
+    else
+        wgrad_reduce_kernel<false><<<sb_div_up(total, 256), 256, 0, st>>>(p.part, p, Cin, o, scale, inv_grad_scale,
+                                                                         nullptr, nonfinite);
     SB_LAUNCHED();
     SB_CHECK_LAUNCH();
     if (o.db) {
@@ -332,7 +344,12 @@ int conv_wgrad(const void* dy16, int dy_ld, const void* x16, int x_ld, int N, in
         colsum_partial_kernel<<<chunks, 256, 0, st>>>(dy32, M, Cout, dy32_ld, rows, bp);
         SB_LAUNCHED();
         SB_CHECK_LAUNCH();
-        colsum_final_kernel<<<sb_div_up(o.rows, 256), 256, 0, st>>>(bp, chunks, Cout, inv_grad_scale, o, nonfinite);
+        if (grad_scale)
+            colsum_final_kernel<true><<<sb_div_up(o.rows, 256), 256, 0, st>>>(bp, chunks, Cout, 0.f, grad_scale, o,
+                                                                             nonfinite);
+        else
+            colsum_final_kernel<false><<<sb_div_up(o.rows, 256), 256, 0, st>>>(bp, chunks, Cout, inv_grad_scale,
+                                                                              nullptr, o, nonfinite);
         SB_LAUNCHED();
         SB_CHECK_LAUNCH();
     }
@@ -349,7 +366,17 @@ extern "C" int sb_conv_wgrad(const void* dy16, const void* x16, int N, int H, in
                              const float* scale, float inv_grad_scale, float* dw, const float* dy32, float* db,
                              int* nonfinite, void* workspace, size_t workspace_bytes, sb_stream_t stream) {
     const WgOut o = {dw, nullptr, db, nullptr, Cout, Cout, 0};
-    return conv_wgrad(dy16, Cout, x16, Cin, N, H, W, Cin, Cout, k, scale, inv_grad_scale, dy32, Cout, o, nonfinite,
+    return conv_wgrad(dy16, Cout, x16, Cin, N, H, W, Cin, Cout, k, scale, inv_grad_scale, nullptr, dy32, Cout, o,
+                      nonfinite, workspace, workspace_bytes, sb_cs(stream));
+}
+
+extern "C" int sb_conv_wgrad_devscale(const void* dy16, const void* x16, int N, int H, int W, int Cin, int Cout, int k,
+                                      const float* scale, const float* grad_scale, float* dw, const float* dy32,
+                                      float* db, int* nonfinite, void* workspace, size_t workspace_bytes,
+                                      sb_stream_t stream) {
+    if (!grad_scale) return SB_EINVAL;
+    const WgOut o = {dw, nullptr, db, nullptr, Cout, Cout, 0};
+    return conv_wgrad(dy16, Cout, x16, Cin, N, H, W, Cin, Cout, k, scale, 0.f, grad_scale, dy32, Cout, o, nonfinite,
                       workspace, workspace_bytes, sb_cs(stream));
 }
 
@@ -363,7 +390,18 @@ extern "C" int sb_conv_wgrad_acc(const void* dy16, int dy_ld, const void* x16, i
                                  float* db_hi, int* nonfinite, void* workspace, size_t workspace_bytes,
                                  sb_stream_t stream) {
     const WgOut o = {dw, dw_hi, db, db_hi, rows, split, accumulate ? 1 : 0};
-    return conv_wgrad(dy16, dy_ld, x16, x_ld, N, H, W, Cin, Cout, k, scale, inv_grad_scale, dy32, dy32_ld, o,
+    return conv_wgrad(dy16, dy_ld, x16, x_ld, N, H, W, Cin, Cout, k, scale, inv_grad_scale, nullptr, dy32, dy32_ld, o,
+                      nonfinite, workspace, workspace_bytes, sb_cs(stream));
+}
+
+extern "C" int sb_conv_wgrad_acc_devscale(const void* dy16, int dy_ld, const void* x16, int x_ld, int N, int H, int W,
+                                          int Cin, int Cout, int k, const float* scale, const float* grad_scale,
+                                          const float* dy32, int dy32_ld, int accumulate, int rows, int split,
+                                          float* dw, float* db, float* dw_hi, float* db_hi, int* nonfinite,
+                                          void* workspace, size_t workspace_bytes, sb_stream_t stream) {
+    if (!grad_scale) return SB_EINVAL;
+    const WgOut o = {dw, dw_hi, db, db_hi, rows, split, accumulate ? 1 : 0};
+    return conv_wgrad(dy16, dy_ld, x16, x_ld, N, H, W, Cin, Cout, k, scale, 0.f, grad_scale, dy32, dy32_ld, o,
                       nonfinite, workspace, workspace_bytes, sb_cs(stream));
 }
 
@@ -400,10 +438,14 @@ __device__ __forceinline__ void fine_range(float r, int y, int n_coarse, int n_f
     while (hi + 1 < n_fine && up_tap(r, hi + 1, n_coarse).i1 <= y) ++hi;
 }
 
-// one block per coarse pixel, threads over channels (fixed summation order: fine rows, then fine columns, ascending)
+// one block per coarse pixel, threads over channels (fixed summation order: fine rows, then fine columns, ascending);
+// DEV_SCALE: scale is read from scale_dev (device, fp32 [1])
+template <bool DEV_SCALE>
 __global__ void fpn_grad_combine_kernel(const float* __restrict__ dp, const float* __restrict__ dt, int N, int H,
                                         int W, int TH, int TW, int C, const float* __restrict__ dp6, int H6, int W6,
-                                        float scale, float* __restrict__ out, __half* __restrict__ out16) {
+                                        float scale, const float* __restrict__ scale_dev, float* __restrict__ out,
+                                        __half* __restrict__ out16) {
+    if (DEV_SCALE) scale = __ldg(scale_dev);
     const int pix = blockIdx.x;
     const int x = pix % W, y = (pix / W) % H, n = pix / (W * H);
     int ylo = 0, yhi = -1, xlo = 0, xhi = -1;
@@ -435,19 +477,36 @@ __global__ void fpn_grad_combine_kernel(const float* __restrict__ dp, const floa
     }
 }
 
-}  // namespace
-
-extern "C" int sb_fpn_grad_combine(const float* dp, const float* dt, int N, int H, int W, int TH, int TW, int C,
-                                   const float* dp6, int H6, int W6, float scale, float* out, void* out16,
-                                   sb_stream_t stream) {
+int fpn_grad_combine(const float* dp, const float* dt, int N, int H, int W, int TH, int TW, int C, const float* dp6,
+                     int H6, int W6, float scale, const float* scale_dev, float* out, void* out16, cudaStream_t st) {
     if (N < 1 || H < 1 || W < 1 || C < 1 || (!out && !out16)) return SB_EINVAL;
     if (dt && (TH < 1 || TW < 1)) return SB_EINVAL;
     if (dp6 && (H6 != (H - 1) / 2 + 1 || W6 != (W - 1) / 2 + 1)) return SB_EINVAL;
     const long long pixels = (long long)N * H * W;
     if (pixels >= 0x7fffffffLL) return SB_EINVAL;
-    fpn_grad_combine_kernel<<<(int)pixels, C < 256 ? C : 256, 0, sb_cs(stream)>>>(
-        dp, dt, N, H, W, TH, TW, C, dp6, H6, W6, scale, out, reinterpret_cast<__half*>(out16));
+    const int threads = C < 256 ? C : 256;
+    if (scale_dev)
+        fpn_grad_combine_kernel<true><<<(int)pixels, threads, 0, st>>>(dp, dt, N, H, W, TH, TW, C, dp6, H6, W6, 0.f,
+                                                                        scale_dev, out, reinterpret_cast<__half*>(out16));
+    else
+        fpn_grad_combine_kernel<false><<<(int)pixels, threads, 0, st>>>(dp, dt, N, H, W, TH, TW, C, dp6, H6, W6, scale,
+                                                                         nullptr, out, reinterpret_cast<__half*>(out16));
     SB_LAUNCHED();
     SB_CHECK_LAUNCH();
     return SB_OK;
+}
+
+}  // namespace
+
+extern "C" int sb_fpn_grad_combine(const float* dp, const float* dt, int N, int H, int W, int TH, int TW, int C,
+                                   const float* dp6, int H6, int W6, float scale, float* out, void* out16,
+                                   sb_stream_t stream) {
+    return fpn_grad_combine(dp, dt, N, H, W, TH, TW, C, dp6, H6, W6, scale, nullptr, out, out16, sb_cs(stream));
+}
+
+extern "C" int sb_fpn_grad_combine_devscale(const float* dp, const float* dt, int N, int H, int W, int TH, int TW,
+                                            int C, const float* dp6, int H6, int W6, const float* scale, float* out,
+                                            void* out16, sb_stream_t stream) {
+    if (!scale) return SB_EINVAL;
+    return fpn_grad_combine(dp, dt, N, H, W, TH, TW, C, dp6, H6, W6, 0.f, scale, out, out16, sb_cs(stream));
 }

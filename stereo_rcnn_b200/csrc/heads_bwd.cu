@@ -54,11 +54,14 @@ __device__ __forceinline__ void box_out(const BoxTailGrad& a, int nc, int o, con
 }
 
 // d pre-activation of RCNN_top.3: dz[r][k] = grad_scale * mask_scale * [fc7[r][k] > 0] * sum_o d[r][o] W[o][k]
-// (o ascending: cls, box, dim); grid (R, K / 256)
+// (o ascending: cls, box, dim); grid (R, K / 256).  DEV_SCALE: grad_scale is read from gs_dev (device, fp32 [1])
+template <bool DEV_SCALE>
 __global__ void __launch_bounds__(256)
 box_tail_dx_kernel(BoxTailGrad a, int nc, const float* __restrict__ fc7, int K, float mask_scale, float gs,
-                   __half* __restrict__ dz16, float* __restrict__ dz32, int* nonfinite) {
+                   const float* __restrict__ gs_dev, __half* __restrict__ dz16, float* __restrict__ dz32,
+                   int* nonfinite) {
     __shared__ float dv[48];
+    if (DEV_SCALE) gs = __ldg(gs_dev);
     const int r = blockIdx.x, tid = threadIdx.x, n_out = 12 * nc;
     if (tid < n_out) {
         const float* d; const float* w; float *dw, *db; int ld, col;
@@ -118,11 +121,15 @@ box_tail_dw_kernel(BoxTailGrad a, int nc, int R, const float* __restrict__ fc7, 
 //   d up[y][x][c] = [up > 0] sum_k w[k][c] dp[k][x]   (the same for every y; stored x grad_scale, fp16, phase-major:
 //                   pixel (y, x) -> (y / 2, x / 2), channel block (y % 2) * 2 + x % 2, the deconv's (a, b) phase)
 //   per-RoI partials: dW[k][c] <- sum_x dp[k][x] colsum[x][c], d deconv bias[c] <- sum_{y,x} d up, sum_x dp[k][x]
+// DEV_SCALE: grad_scale is read from gs_dev (device, fp32 [1])
+template <bool DEV_SCALE>
 __global__ void __launch_bounds__(1024)
 kpts_tail_bwd_kernel(const __half* __restrict__ up, int G, int C, const float* __restrict__ w,
                      const float* __restrict__ d_kp, const float* __restrict__ d_lb, const float* __restrict__ d_rb,
-                     float gs, __half* __restrict__ dup, float* __restrict__ part, int part_ld, int* nonfinite) {
+                     float gs, const float* __restrict__ gs_dev, __half* __restrict__ dup, float* __restrict__ part,
+                     int part_ld, int* nonfinite) {
     extern __shared__ float dp[];       // [6][G]
+    if (DEV_SCALE) gs = __ldg(gs_dev);
     const int r = blockIdx.x, c = threadIdx.x, Gh = G / 2;
     for (int i = c; i < 6 * G; i += blockDim.x) {
         const int k = i / G, x = i % G;
@@ -197,6 +204,70 @@ int grid_for(long long n) { return (int)(n < 256LL * 4 * 132 * 8 ? (n + 255) / 2
 
 size_t kpts_part_ld(int C) { return (size_t)7 * C + 8; }
 
+// grad_scale_dev (device, may be NULL): the gradient scale read on the device in place of grad_scale
+int box_tail_backward(const float* d_cls_score, const float* d_bbox_pred, const float* d_dim_orien_pred,
+                      const float* fc7, int R, int K, int n_classes, const float* w_cls, const float* w_box,
+                      const float* w_dim, float mask_scale, float grad_scale, const float* grad_scale_dev, float* dw_cls,
+                      float* db_cls, float* dw_box, float* db_box, float* dw_dim, float* db_dim, void* dz16, float* dz32,
+                      int* nonfinite, cudaStream_t st) {
+    if (R < 1 || K < 1 || n_classes < 1 || n_classes > 4) return SB_EINVAL;
+    if (!(mask_scale > 0.f) || !isfinite(mask_scale)) return SB_EINVAL;
+    if (!grad_scale_dev && (!(grad_scale > 0.f) || !isfinite(grad_scale))) return SB_EINVAL;
+    const void* need[] = {d_cls_score, d_bbox_pred, d_dim_orien_pred, fc7, w_cls, w_box, w_dim, dw_cls, db_cls,
+                          dw_box, db_box, dw_dim, db_dim, dz16, dz32};
+    for (const void* q : need)
+        if (!q) return SB_EINVAL;
+    if (misaligned(dz16, 2)) return SB_EINVAL;
+    if ((long long)R * K >= 0x7fffffffLL) return SB_EINVAL;
+    BoxTailGrad a = {d_cls_score, d_bbox_pred, d_dim_orien_pred, w_cls, w_box, w_dim,
+                     dw_cls, db_cls, dw_box, db_box, dw_dim, db_dim};
+    const dim3 grid(R, sb_div_up(K, 256));
+    if (grad_scale_dev)
+        box_tail_dx_kernel<true><<<grid, 256, 0, st>>>(a, n_classes, fc7, K, mask_scale, 0.f, grad_scale_dev,
+                                                       reinterpret_cast<__half*>(dz16), dz32, nonfinite);
+    else
+        box_tail_dx_kernel<false><<<grid, 256, 0, st>>>(a, n_classes, fc7, K, mask_scale, grad_scale, nullptr,
+                                                        reinterpret_cast<__half*>(dz16), dz32, nonfinite);
+    SB_LAUNCHED();
+    SB_CHECK_LAUNCH();
+    box_tail_dw_kernel<<<dim3(sb_div_up(K, 256), 12 * n_classes), 256, 0, st>>>(a, n_classes, R, fc7, K, nonfinite);
+    SB_LAUNCHED();
+    SB_CHECK_LAUNCH();
+    return SB_OK;
+}
+
+int kpts_tail_backward(const void* up16, int R, int G, int C, const float* w, const float* d_kpts_pred,
+                       const float* d_left_border_pred, const float* d_right_border_pred, float grad_scale,
+                       const float* grad_scale_dev, void* dup16, float* dw, float* db, float* db_up, int* nonfinite,
+                       void* workspace, size_t workspace_bytes, cudaStream_t st) {
+    if (R < 1 || G < 2 || G > 64 || (G & 1) || C < 32 || C > 1024 || (C & 31)) return SB_EINVAL;
+    if (!grad_scale_dev && (!(grad_scale > 0.f) || !isfinite(grad_scale))) return SB_EINVAL;
+    const void* need[] = {up16, w, d_kpts_pred, d_left_border_pred, d_right_border_pred, dup16, dw, db, db_up,
+                          workspace};
+    for (const void* q : need)
+        if (!q) return SB_EINVAL;
+    if (misaligned(up16, 2) || misaligned(dup16, 2) || misaligned(workspace, 4)) return SB_EINVAL;
+    if (workspace_bytes < (size_t)R * kpts_part_ld(C) * sizeof(float)) return SB_EINVAL;
+    const int part_ld = (int)kpts_part_ld(C);
+    float* part = reinterpret_cast<float*>(workspace);
+    const size_t smem = 6 * G * sizeof(float);
+    if (grad_scale_dev)
+        kpts_tail_bwd_kernel<true><<<R, C, smem, st>>>(
+            reinterpret_cast<const __half*>(up16), G, C, w, d_kpts_pred, d_left_border_pred, d_right_border_pred,
+            0.f, grad_scale_dev, reinterpret_cast<__half*>(dup16), part, part_ld, nonfinite);
+    else
+        kpts_tail_bwd_kernel<false><<<R, C, smem, st>>>(
+            reinterpret_cast<const __half*>(up16), G, C, w, d_kpts_pred, d_left_border_pred, d_right_border_pred,
+            grad_scale, nullptr, reinterpret_cast<__half*>(dup16), part, part_ld, nonfinite);
+    SB_LAUNCHED();
+    SB_CHECK_LAUNCH();
+    kpts_tail_bwd_reduce_kernel<<<sb_div_up(7 * C + 6, 256), 256, 0, st>>>(part, part_ld, R, C, G, dw, db, db_up,
+                                                                            nonfinite);
+    SB_LAUNCHED();
+    SB_CHECK_LAUNCH();
+    return SB_OK;
+}
+
 }  // namespace
 
 extern "C" int sb_dropout_words(void* x, int x_is_half, long long n, const unsigned* words, double p,
@@ -230,25 +301,21 @@ extern "C" int sb_box_tail_backward(const float* d_cls_score, const float* d_bbo
                                     const float* w_box, const float* w_dim, float mask_scale, float grad_scale,
                                     float* dw_cls, float* db_cls, float* dw_box, float* db_box, float* dw_dim,
                                     float* db_dim, void* dz16, float* dz32, int* nonfinite, sb_stream_t stream) {
-    if (R < 1 || K < 1 || n_classes < 1 || n_classes > 4) return SB_EINVAL;
-    if (!(mask_scale > 0.f) || !isfinite(mask_scale) || !(grad_scale > 0.f) || !isfinite(grad_scale)) return SB_EINVAL;
-    const void* need[] = {d_cls_score, d_bbox_pred, d_dim_orien_pred, fc7, w_cls, w_box, w_dim, dw_cls, db_cls,
-                          dw_box, db_box, dw_dim, db_dim, dz16, dz32};
-    for (const void* q : need)
-        if (!q) return SB_EINVAL;
-    if (misaligned(dz16, 2)) return SB_EINVAL;
-    if ((long long)R * K >= 0x7fffffffLL) return SB_EINVAL;
-    BoxTailGrad a = {d_cls_score, d_bbox_pred, d_dim_orien_pred, w_cls, w_box, w_dim,
-                     dw_cls, db_cls, dw_box, db_box, dw_dim, db_dim};
-    const cudaStream_t st = sb_cs(stream);
-    box_tail_dx_kernel<<<dim3(R, sb_div_up(K, 256)), 256, 0, st>>>(a, n_classes, fc7, K, mask_scale, grad_scale,
-                                                                    reinterpret_cast<__half*>(dz16), dz32, nonfinite);
-    SB_LAUNCHED();
-    SB_CHECK_LAUNCH();
-    box_tail_dw_kernel<<<dim3(sb_div_up(K, 256), 12 * n_classes), 256, 0, st>>>(a, n_classes, R, fc7, K, nonfinite);
-    SB_LAUNCHED();
-    SB_CHECK_LAUNCH();
-    return SB_OK;
+    return box_tail_backward(d_cls_score, d_bbox_pred, d_dim_orien_pred, fc7, R, K, n_classes, w_cls, w_box, w_dim,
+                             mask_scale, grad_scale, nullptr, dw_cls, db_cls, dw_box, db_box, dw_dim, db_dim, dz16,
+                             dz32, nonfinite, sb_cs(stream));
+}
+
+extern "C" int sb_box_tail_backward_devscale(const float* d_cls_score, const float* d_bbox_pred,
+                                             const float* d_dim_orien_pred, const float* fc7, int R, int K,
+                                             int n_classes, const float* w_cls, const float* w_box, const float* w_dim,
+                                             float mask_scale, const float* grad_scale, float* dw_cls, float* db_cls,
+                                             float* dw_box, float* db_box, float* dw_dim, float* db_dim, void* dz16,
+                                             float* dz32, int* nonfinite, sb_stream_t stream) {
+    if (!grad_scale) return SB_EINVAL;
+    return box_tail_backward(d_cls_score, d_bbox_pred, d_dim_orien_pred, fc7, R, K, n_classes, w_cls, w_box, w_dim,
+                             mask_scale, 0.f, grad_scale, dw_cls, db_cls, dw_box, db_box, dw_dim, db_dim, dz16, dz32,
+                             nonfinite, sb_cs(stream));
 }
 
 extern "C" size_t sb_kpts_tail_backward_workspace(int R, int C) {
@@ -260,27 +327,18 @@ extern "C" int sb_kpts_tail_backward(const void* up16, int R, int G, int C, cons
                                      const float* d_left_border_pred, const float* d_right_border_pred,
                                      float grad_scale, void* dup16, float* dw, float* db, float* db_up, int* nonfinite,
                                      void* workspace, size_t workspace_bytes, sb_stream_t stream) {
-    if (R < 1 || G < 2 || G > 64 || (G & 1) || C < 32 || C > 1024 || (C & 31)) return SB_EINVAL;
-    if (!(grad_scale > 0.f) || !isfinite(grad_scale)) return SB_EINVAL;
-    const void* need[] = {up16, w, d_kpts_pred, d_left_border_pred, d_right_border_pred, dup16, dw, db, db_up,
-                          workspace};
-    for (const void* q : need)
-        if (!q) return SB_EINVAL;
-    if (misaligned(up16, 2) || misaligned(dup16, 2) || misaligned(workspace, 4)) return SB_EINVAL;
-    if (workspace_bytes < sb_kpts_tail_backward_workspace(R, C)) return SB_EINVAL;
-    const int part_ld = (int)kpts_part_ld(C);
-    const cudaStream_t st = sb_cs(stream);
-    float* part = reinterpret_cast<float*>(workspace);
-    kpts_tail_bwd_kernel<<<R, C, 6 * G * sizeof(float), st>>>(
-        reinterpret_cast<const __half*>(up16), G, C, w, d_kpts_pred, d_left_border_pred, d_right_border_pred,
-        grad_scale, reinterpret_cast<__half*>(dup16), part, part_ld, nonfinite);
-    SB_LAUNCHED();
-    SB_CHECK_LAUNCH();
-    kpts_tail_bwd_reduce_kernel<<<sb_div_up(7 * C + 6, 256), 256, 0, st>>>(part, part_ld, R, C, G, dw, db, db_up,
-                                                                            nonfinite);
-    SB_LAUNCHED();
-    SB_CHECK_LAUNCH();
-    return SB_OK;
+    return kpts_tail_backward(up16, R, G, C, w, d_kpts_pred, d_left_border_pred, d_right_border_pred, grad_scale,
+                              nullptr, dup16, dw, db, db_up, nonfinite, workspace, workspace_bytes, sb_cs(stream));
+}
+
+extern "C" int sb_kpts_tail_backward_devscale(const void* up16, int R, int G, int C, const float* w,
+                                              const float* d_kpts_pred, const float* d_left_border_pred,
+                                              const float* d_right_border_pred, const float* grad_scale, void* dup16,
+                                              float* dw, float* db, float* db_up, int* nonfinite, void* workspace,
+                                              size_t workspace_bytes, sb_stream_t stream) {
+    if (!grad_scale) return SB_EINVAL;
+    return kpts_tail_backward(up16, R, G, C, w, d_kpts_pred, d_left_border_pred, d_right_border_pred, 0.f, grad_scale,
+                              dup16, dw, db, db_up, nonfinite, workspace, workspace_bytes, sb_cs(stream));
 }
 
 extern "C" int sb_permute3(const float* src, int d0, int d1, int d2, long long s0, long long s1, long long s2,

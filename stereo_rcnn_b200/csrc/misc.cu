@@ -25,6 +25,14 @@ fill_kernel(float4* __restrict__ p, size_t n4, float v) {
     for (; i < n4; i += stride) p[i] = f;
 }
 
+// p[i] = 1 / *v (one IEEE division, exact when *v is a power of two)
+__global__ void __launch_bounds__(256)
+fill_reciprocal_kernel(float* __restrict__ p, size_t n, const float* __restrict__ v) {
+    const float r = 1.0f / __ldg(v);
+    const size_t stride = (size_t)gridDim.x * 256;
+    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n; i += stride) p[i] = r;
+}
+
 // nn.MaxPool2d(kernel_size=3, stride=2, padding=0, ceil_mode=True) (resnet.py:113), NHWC
 __global__ void __launch_bounds__(256)
 maxpool_kernel(const float4* __restrict__ in, int N, int H, int W, int C4, int Ho, int Wo,
@@ -392,6 +400,16 @@ extern "C" int sb_fill(float* p, size_t n, float v, sb_stream_t stream) {
     if (n == 0) return SB_OK;
     if (n & 3) return SB_EINVAL;
     fill_kernel<<<148 * 8, 256, 0, sb_cs(stream)>>>((float4*)p, n / 4, v);
+    SB_LAUNCHED();
+    SB_CHECK_LAUNCH();
+    return SB_OK;
+}
+
+extern "C" int sb_fill_reciprocal(float* p, size_t n, const float* v, sb_stream_t stream) {
+    if (!v || (n > 0 && !p)) return SB_EINVAL;
+    if (n == 0) return SB_OK;
+    const size_t blocks = (n + 255) / 256;
+    fill_reciprocal_kernel<<<(unsigned)(blocks < 148 * 8 ? blocks : 148 * 8), 256, 0, sb_cs(stream)>>>(p, n, v);
     SB_LAUNCHED();
     SB_CHECK_LAUNCH();
     return SB_OK;

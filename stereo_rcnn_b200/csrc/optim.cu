@@ -3,6 +3,8 @@
 //
 //   sb_sgd_step      torch.optim.SGD.step (trainval_net.py:168,227), dampening 0, no Nesterov: multi-tensor, the
 //                    learning rate read on the device, skipped when the backward raised found_inf
+//   sb_loss_scale_update  torch.cuda.amp.GradScaler.update (_amp_update_scale_) on the same found_inf: the dynamic
+//                    loss scale backed off or grown on the device, held within [2^-32, 2^32]
 //   sb_pack_plan     validate a table of pack targets and assign its tiles
 //   sb_pack_weights  rewrite every derived copy of a table (K-major, TF32-rounded, fp16, transposed and flipped, frozen-BN
 //                    scale folded) from the fp32 masters in one launch
@@ -77,6 +79,33 @@ sgd_step_kernel(const SgdChunk c, const float* __restrict__ lr, float momentum, 
         P[j] = p;
         M[j] = m;
     }
+}
+
+// --------------------------------------------------------------------------------------------- dynamic loss scale
+constexpr float kMaxLossScale = 4294967296.0f, kMinLossScale = 1.0f / 4294967296.0f;    // 2^32, 2^-32
+
+__global__ void loss_scale_update_kernel(const int* __restrict__ found_inf, float* __restrict__ scale,
+                                         int* __restrict__ tracker, float growth, float backoff, int interval) {
+    float s = *scale;
+    if (*found_inf != 0) {
+        s = fmaxf(s * backoff, kMinLossScale);
+        *tracker = 0;
+    } else {
+        const int t = *tracker + 1;
+        if (t >= interval) {
+            const float g = s * growth;
+            if (g <= kMaxLossScale) s = g;        // a growth past the top leaves the scale, as torch a non-finite one
+            *tracker = 0;
+        } else {
+            *tracker = t;
+        }
+    }
+    *scale = s;
+}
+
+bool power_of_two(float v) {
+    int e;
+    return v > 0.f && isfinite(v) && frexpf(v, &e) == 0.5f;
 }
 
 // --------------------------------------------------------------------------------------------- weight packing
@@ -245,6 +274,19 @@ extern "C" int sb_sgd_step(float* const* params, float* const* grads, float* con
         sgd_step_kernel<<<blocks, kSgdThreads, 0, st>>>(c, lr, momentum, skip, skipped, base == 0);
         SB_LAUNCHED();
     }
+    SB_CHECK_LAUNCH();
+    return SB_OK;
+}
+
+extern "C" int sb_loss_scale_update(const int* found_inf, float* scale, int* growth_tracker, float growth_factor,
+                                    float backoff_factor, int growth_interval, sb_stream_t stream) {
+    if (!found_inf || !scale || !growth_tracker || growth_interval < 1) return SB_EINVAL;
+    if (!power_of_two(growth_factor) || !(growth_factor > 1.f) || !power_of_two(backoff_factor) ||
+        !(backoff_factor < 1.f))
+        return SB_EINVAL;
+    loss_scale_update_kernel<<<1, 1, 0, sb_cs(stream)>>>(found_inf, scale, growth_tracker, growth_factor,
+                                                         backoff_factor, growth_interval);
+    SB_LAUNCHED();
     SB_CHECK_LAUNCH();
     return SB_OK;
 }

@@ -343,12 +343,16 @@ rpn_head_scores_kernel(const float* __restrict__ head, long long total_pix, int 
 }
 
 // backward of the fused head's outputs: dhead[p][0..5] = s * d_cls[p*6 ..], dhead[p][6..23] = s * d_box[p*18 ..],
-// columns 24..63 zero (K padding of the head's data gradient and Cout padding of its weight gradient)
+// columns 24..63 zero (K padding of the head's data gradient and Cout padding of its weight gradient); DEV_SCALE: s is
+// read from grad_scale_dev (device, fp32 [1])
+template <bool DEV_SCALE>
 __global__ void __launch_bounds__(256)
 rpn_head_grad_kernel(const float* __restrict__ d_cls, const float* __restrict__ d_box, long long total_pix,
-                     float grad_scale, __half* __restrict__ dhead16, float* __restrict__ dhead32) {
+                     float grad_scale, const float* __restrict__ grad_scale_dev, __half* __restrict__ dhead16,
+                     float* __restrict__ dhead32) {
     const long long e = (long long)blockIdx.x * 256 + threadIdx.x;
     if (e >= total_pix * 64) return;
+    if (DEV_SCALE) grad_scale = __ldg(grad_scale_dev);
     const long long p = e >> 6;
     const int c = (int)(e & 63);
     float v = 0.f;
@@ -538,15 +542,34 @@ extern "C" int sb_rpn_head_scores(const float* head, int B, int P, int ld, float
     return SB_OK;
 }
 
-extern "C" int sb_rpn_head_grad(const float* d_cls_score, const float* d_bbox_pred, int B, int P, float grad_scale,
-                                void* dhead16, float* dhead32, sb_stream_t stream) {
+namespace {
+
+int rpn_head_grad(const float* d_cls_score, const float* d_bbox_pred, int B, int P, float grad_scale,
+                  const float* grad_scale_dev, void* dhead16, float* dhead32, cudaStream_t st) {
     const long long total = (long long)B * P;
     if (B < 0 || P < 0 || (total > 0 && (!d_cls_score || !d_bbox_pred || !dhead16))) return SB_EINVAL;
     if ((reinterpret_cast<uintptr_t>(dhead16) & 1) || (reinterpret_cast<uintptr_t>(dhead32) & 3)) return SB_EINVAL;
     if (total == 0) return SB_OK;
-    rpn_head_grad_kernel<<<sb_div_up(total * 64, 256), 256, 0, sb_cs(stream)>>>(
-        d_cls_score, d_bbox_pred, total, grad_scale, reinterpret_cast<__half*>(dhead16), dhead32);
+    if (grad_scale_dev)
+        rpn_head_grad_kernel<true><<<sb_div_up(total * 64, 256), 256, 0, st>>>(
+            d_cls_score, d_bbox_pred, total, 0.f, grad_scale_dev, reinterpret_cast<__half*>(dhead16), dhead32);
+    else
+        rpn_head_grad_kernel<false><<<sb_div_up(total * 64, 256), 256, 0, st>>>(
+            d_cls_score, d_bbox_pred, total, grad_scale, nullptr, reinterpret_cast<__half*>(dhead16), dhead32);
     SB_LAUNCHED();
     SB_CHECK_LAUNCH();
     return SB_OK;
+}
+
+}  // namespace
+
+extern "C" int sb_rpn_head_grad(const float* d_cls_score, const float* d_bbox_pred, int B, int P, float grad_scale,
+                                void* dhead16, float* dhead32, sb_stream_t stream) {
+    return rpn_head_grad(d_cls_score, d_bbox_pred, B, P, grad_scale, nullptr, dhead16, dhead32, sb_cs(stream));
+}
+
+extern "C" int sb_rpn_head_grad_devscale(const float* d_cls_score, const float* d_bbox_pred, int B, int P,
+                                         const float* grad_scale, void* dhead16, float* dhead32, sb_stream_t stream) {
+    if (!grad_scale) return SB_EINVAL;
+    return rpn_head_grad(d_cls_score, d_bbox_pred, B, P, 0.f, grad_scale, dhead16, dhead32, sb_cs(stream));
 }

@@ -481,12 +481,14 @@ class StereoRCNNEngine(object):
         NHWC, the shapes trunk_fpn returns; left and right images batched, so every weight gradient sums over both).
         Returns {state_dict name: fp32 gradient} of exactly trainable_trunk_fpn_params(fixed_blocks), in the
         reference's layout; tensors given in `grads` (e.g. GradientBuckets views) are written in place.
-        grad_scale (a power of two) multiplies dP before the fp16 chain and is divided out of the results exactly;
-        found_inf is set when a result is not finite; clear_found_inf=False keeps a flag an earlier backward of the
-        same step set (rpn_backward before this).  No host synchronisation: graph-capturable."""
+        grad_scale (a power of two) multiplies dP before the fp16 chain and is divided out of the results exactly; it is
+        a host float, or an fp32 [1] CUDA tensor that every kernel reads on the device (a captured backward then follows
+        a scale changed between replays).  found_inf is set when a result is not finite; clear_found_inf=False keeps a
+        flag an earlier backward of the same step set (rpn_backward before this).  No host synchronisation:
+        graph-capturable."""
         self._pack_backward()
         dev = self.device
-        gs = float(grad_scale)
+        gs = grad_scale if ops.device_scale(grad_scale) else float(grad_scale)
         out = self._grad_buffers(trainable_trunk_fpn_params(fixed_blocks), grads)
         if clear_found_inf:
             ops.fill_(self._found_inf, 0.0)
@@ -590,18 +592,24 @@ class StereoRCNNEngine(object):
         trainable_rpn_params(), in the reference's layout; tensors given in `grads` are written in place,
         {"p2".."p6": dP fp32 [2B,h,w,256]} for trunk_fpn_backward).  Weight gradients are summed over the levels
         P2..P6 and, for RPN_Conv, left before right: a fixed order, bit-identical run to run.  grad_scale (a power of
-        two) scales the fp16 chain and is divided out of every result exactly; found_inf is cleared, then set when a
-        gradient is not finite.  No host synchronisation: graph-capturable."""
+        two; a host float or an fp32 [1] CUDA tensor, as in trunk_fpn_backward) scales the fp16 chain and is divided out
+        of every result exactly; found_inf is cleared, then set when a gradient is not finite.  No host
+        synchronisation: graph-capturable."""
         self._pack_backward()
         dev = self.device
-        gs = float(grad_scale)
+        on_dev = ops.device_scale(grad_scale)
+        gs = grad_scale if on_dev else float(grad_scale)
         B, offs = saved.B, saved.offs
         P = offs[-1]
         out = self._grad_buffers(trainable_rpn_params(), grads)
         ops.fill_(self._found_inf, 0.0)
         dh16, dh32 = ops.rpn_head_grad(d_cls_score, d_bbox_pred, B, P, gs)
-        # the dgrad epilogue's per-channel scale divides grad_scale out of dP (exact: a power of two)
-        unscale = ops.fill_(torch.empty(256, dtype=torch.float32, device=dev), 1.0 / gs) if gs != 1.0 else None
+        # the dgrad epilogue's per-channel scale divides grad_scale out of dP (exact: a power of two); a device scale
+        # is inverted on the device
+        if on_dev:
+            unscale = ops.fill_reciprocal_(torch.empty(256, dtype=torch.float32, device=dev), gs)
+        else:
+            unscale = ops.fill_(torch.empty(256, dtype=torch.float32, device=dev), 1.0 / gs) if gs != 1.0 else None
         hd, cd = self._bwd["rpn_heads"], self._bwd["RCNN_rpn.RPN_Conv"]
         w_cls, w_box = out["RCNN_rpn.RPN_cls_score.weight"], out["RCNN_rpn.RPN_bbox_pred_left_right.weight"]
         b_cls, b_box = out["RCNN_rpn.RPN_cls_score.bias"], out["RCNN_rpn.RPN_bbox_pred_left_right.bias"]
@@ -730,21 +738,27 @@ class StereoRCNNEngine(object):
         layout; tensors given in `grads` are written in place,
         {"pooled_box": fp32 [R,7,7,512] (channels 0..255 the left image, 256..511 the right),
          "pooled_kpts": fp32 [R,14,14,256]}: the gradients of the two pooled tensors).
-        Every sum runs in a fixed order: bit-identical run to run.  grad_scale (a power of two) scales the fp16 chain
-        and is divided out of every result exactly; found_inf is cleared, then set when a gradient is not finite;
+        Every sum runs in a fixed order: bit-identical run to run.  grad_scale (a power of two; a host float or an fp32
+        [1] CUDA tensor, as in trunk_fpn_backward) scales the fp16 chain and is divided out of every result exactly;
+        found_inf is cleared, then set when a gradient is not finite;
         clear_found_inf=False keeps a flag an earlier backward of the same step set (rpn_backward before this).
         No host synchronisation: graph-capturable."""
         self._pack_heads_backward()
         dev = self.device
-        gs = float(grad_scale)
+        on_dev = ops.device_scale(grad_scale)
+        gs = grad_scale if on_dev else float(grad_scale)
         R = saved.R
         out = self._grad_buffers(trainable_rcnn_head_params(self.n_classes), grads)
         nf = self._found_inf
         if clear_found_inf:
             ops.fill_(nf, 0.0)
         f32 = lambda *sh: torch.empty(*sh, dtype=torch.float32, device=dev)
-        # the dgrad epilogue's per-channel scale divides grad_scale out of the pooled gradients (exact: a power of two)
-        unscale = ops.fill_(f32(2048), 1.0 / gs) if gs != 1.0 else None
+        # the dgrad epilogue's per-channel scale divides grad_scale out of the pooled gradients (exact: a power of two);
+        # a device scale is inverted on the device
+        if on_dev:
+            unscale = ops.fill_reciprocal_(f32(2048), gs)
+        else:
+            unscale = ops.fill_(f32(2048), 1.0 / gs) if gs != 1.0 else None
         # ---- box head: the three linears (fp32), then RCNN_top.3 and RCNN_top.0 as 1x1 convs over the R RoIs
         keep = 1.0 / (1.0 - DROPOUT_P) if saved.dropout else 1.0
         w_cls, _, w_box, _, w_dim, _ = self.fc

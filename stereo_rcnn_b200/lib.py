@@ -118,6 +118,19 @@ _SIGS = {
     "sb_conv_wgrad_acc_workspace": (c_size_t, [c_int] * 6),
     "sb_conv_wgrad_acc": (c_int, [c_void_p, c_int, c_void_p] + [c_int] * 7 + [c_void_p, c_float, c_void_p] +
                           [c_int] * 4 + [c_void_p] * 6 + [c_size_t, c_void_p]),
+    # the same six with the gradient scale fp32 [1] in device memory
+    "sb_conv_wgrad_devscale": (c_int, [c_void_p, c_void_p] + [c_int] * 6 + [c_void_p] * 6 + [c_void_p, c_size_t,
+                                                                                            c_void_p]),
+    "sb_conv_wgrad_acc_devscale": (c_int, [c_void_p, c_int, c_void_p] + [c_int] * 7 + [c_void_p] * 3 + [c_int] * 4 +
+                                   [c_void_p] * 6 + [c_size_t, c_void_p]),
+    "sb_fpn_grad_combine_devscale": (c_int, [c_void_p, c_void_p] + [c_int] * 6 + [c_void_p, c_int, c_int] +
+                                     [c_void_p] * 4),
+    "sb_rpn_head_grad_devscale": (c_int, [c_void_p, c_void_p, c_int, c_int] + [c_void_p] * 4),
+    "sb_box_tail_backward_devscale": (c_int, [c_void_p] * 4 + [c_int, c_int, c_int] + [c_void_p] * 3 +
+                                      [c_float, c_void_p] + [c_void_p] * 9 + [c_void_p]),
+    "sb_kpts_tail_backward_devscale": (c_int, [c_void_p, c_int, c_int, c_int] + [c_void_p] * 11 +
+                                       [c_size_t, c_void_p]),
+    "sb_fill_reciprocal": (c_int, [c_void_p, c_size_t, c_void_p, c_void_p]),
     "sb_box_tail_scores": (c_int, [c_void_p, c_int, c_int, c_int] + [c_void_p] * 10 + [c_void_p]),
     "sb_kpts_logits": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "sb_dropout_words": (c_int, [c_void_p, c_int, c_ll, c_void_p, c_double, c_void_p]),
@@ -172,6 +185,7 @@ _SIGS = {
     # the optimizer step and the device-side weight refresh
     "sb_sgd_step": (c_int, [ctypes.POINTER(c_void_p)] * 3 + [ctypes.POINTER(c_size_t), ctypes.POINTER(c_float),
                             ctypes.POINTER(c_float), c_int, c_void_p, c_float, c_void_p, c_void_p, c_void_p]),
+    "sb_loss_scale_update": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_float, c_int, c_void_p]),
     "sb_pack_plan": (c_int, [ctypes.POINTER(PackTarget), c_int, ctypes.POINTER(c_ll)]),
     "sb_pack_weights": (c_int, [ctypes.POINTER(PackTarget), c_void_p, c_int, c_void_p]),
     # the training side of the input pipeline

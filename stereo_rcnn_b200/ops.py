@@ -496,10 +496,21 @@ def conv2d_dgrad(desc, mask16=None):
     check(L.sb_conv2d_tc_dgrad(ctypes.byref(desc), ptr(mask16), stream_ptr()), "sb_conv2d_tc_dgrad")
 
 
+def device_scale(grad_scale):
+    """True when grad_scale is a loss scale that lives on the device (fp32 [1] CUDA tensor, read by the _devscale entry
+    points), False for a host float"""
+    if not torch.is_tensor(grad_scale):
+        return False
+    assert grad_scale.dtype == torch.float32 and grad_scale.is_cuda and grad_scale.numel() == 1 and \
+        grad_scale.is_contiguous(), "a device grad_scale is an fp32 [1] CUDA tensor"
+    return True
+
+
 def conv_wgrad(dy16, x16, k, dw, scale=None, grad_scale=1.0, dy32=None, db=None, nonfinite=None):
     """weight (and bias) gradient of a k x k (pad k // 2) stride-1 conv: dy16 [N,H,W,Cout], x16 [N,H,W,Cin] fp16 NHWC
     -> dw [Cout,Cin,k,k] = scale[co] / grad_scale * sum dy x, db [Cout] = sum dy32 / grad_scale (fp32, written in
-    place); nonfinite: int32 [1] device flag set to 1 on a non-finite result"""
+    place); nonfinite: int32 [1] device flag set to 1 on a non-finite result.  grad_scale: a host float, or an fp32 [1]
+    CUDA tensor read on the device (sb_conv_wgrad_devscale)"""
     L = _l.load()
     N, H, W, Cout = dy16.shape
     Cin = x16.shape[3]
@@ -507,8 +518,13 @@ def conv_wgrad(dy16, x16, k, dw, scale=None, grad_scale=1.0, dy32=None, db=None,
     assert tuple(dw.shape) == (Cout, Cin, k, k) and dw.dtype == torch.float32
     nb = L.sb_conv_wgrad_workspace(N, H, W, Cin, Cout, k)
     ws = workspace(nb, dy16.device, "wgrad")
-    check(L.sb_conv_wgrad(ptr(dy16), ptr(x16), N, H, W, Cin, Cout, k, ptr(scale), float(1.0 / grad_scale), ptr(dw),
-                          ptr(dy32), ptr(db), ptr(nonfinite), ptr(ws), nb, stream_ptr()), "sb_conv_wgrad")
+    if device_scale(grad_scale):
+        check(L.sb_conv_wgrad_devscale(ptr(dy16), ptr(x16), N, H, W, Cin, Cout, k, ptr(scale), ptr(grad_scale),
+                                       ptr(dw), ptr(dy32), ptr(db), ptr(nonfinite), ptr(ws), nb, stream_ptr()),
+              "sb_conv_wgrad_devscale")
+    else:
+        check(L.sb_conv_wgrad(ptr(dy16), ptr(x16), N, H, W, Cin, Cout, k, ptr(scale), float(1.0 / grad_scale),
+                              ptr(dw), ptr(dy32), ptr(db), ptr(nonfinite), ptr(ws), nb, stream_ptr()), "sb_conv_wgrad")
     return dw, db
 
 
@@ -524,7 +540,7 @@ def conv_wgrad_acc(dy16, x16, k, dw, db=None, dy32=None, scale=None, grad_scale=
                    split=None, dw_hi=None, db_hi=None, nonfinite=None):
     """conv_wgrad on NHWC views whose pixels are rows of one pitch (dy16 may be a channel slice of a wider tensor),
     optionally added to dw / db (accumulate=True).  Rows [0, split) of dW / db go to dw / db, rows [split, rows) to
-    dw_hi / db_hi, rows past `rows` are dropped (defaults: rows = split = Cout)."""
+    dw_hi / db_hi, rows past `rows` are dropped (defaults: rows = split = Cout).  grad_scale as in conv_wgrad."""
     L = _l.load()
     N, H, W, Cout = dy16.shape
     Cin = x16.shape[3]
@@ -540,11 +556,13 @@ def conv_wgrad_acc(dy16, x16, k, dw, db=None, dy32=None, scale=None, grad_scale=
     assert dy32 is None or (dy32.dtype == torch.float32 and tuple(dy32.shape) == (N, H, W, Cout))
     nb = L.sb_conv_wgrad_acc_workspace(N, H, W, Cin, Cout, k)
     ws = workspace(nb, dy16.device, "wgrad")
-    check(L.sb_conv_wgrad_acc(_vptr(dy16), _flat_rows_ld(dy16), _vptr(x16), _flat_rows_ld(x16), N, H, W, Cin, Cout, k,
-                              ptr(scale), float(1.0 / grad_scale), _vptr(dy32),
-                              _flat_rows_ld(dy32) if dy32 is not None else 0, int(bool(accumulate)), rows, split,
-                              ptr(dw), ptr(db), ptr(dw_hi), ptr(db_hi), ptr(nonfinite), ptr(ws), nb, stream_ptr()),
-          "sb_conv_wgrad_acc")
+    dev = device_scale(grad_scale)
+    fn, name = (L.sb_conv_wgrad_acc_devscale, "sb_conv_wgrad_acc_devscale") if dev else \
+        (L.sb_conv_wgrad_acc, "sb_conv_wgrad_acc")
+    check(fn(_vptr(dy16), _flat_rows_ld(dy16), _vptr(x16), _flat_rows_ld(x16), N, H, W, Cin, Cout, k, ptr(scale),
+             ptr(grad_scale) if dev else float(1.0 / grad_scale), _vptr(dy32),
+             _flat_rows_ld(dy32) if dy32 is not None else 0, int(bool(accumulate)), rows, split, ptr(dw), ptr(db),
+             ptr(dw_hi), ptr(db_hi), ptr(nonfinite), ptr(ws), nb, stream_ptr()), name)
     return dw, db
 
 
@@ -558,21 +576,26 @@ def rpn_head_scores(head, B, P):
 
 def rpn_head_grad(d_cls_score, d_bbox_pred, B, P, grad_scale=1.0, f32=True):
     """d rpn_cls_score [B,3P,2], d rpn_bbox_pred [B,3P,6] -> (dhead16 [B,P,64] fp16, dhead32 [B,P,64] fp32 or None):
-    grad_scale * d in the fused head's rows 0..23, zero in 24..63"""
+    grad_scale * d in the fused head's rows 0..23, zero in 24..63 (grad_scale as in conv_wgrad)"""
     L = _l.load()
     assert tuple(d_cls_score.shape) == (B, 3 * P, 2) and tuple(d_bbox_pred.shape) == (B, 3 * P, 6)
     dev = d_cls_score.device
     dh16 = torch.empty(B, P, 64, dtype=torch.float16, device=dev)
     dh32 = torch.empty(B, P, 64, dtype=torch.float32, device=dev) if f32 else None
-    check(L.sb_rpn_head_grad(ptr(_f32c(d_cls_score)), ptr(_f32c(d_bbox_pred)), B, P, float(grad_scale), ptr(dh16),
-                             ptr(dh32), stream_ptr()), "sb_rpn_head_grad")
+    if device_scale(grad_scale):
+        check(L.sb_rpn_head_grad_devscale(ptr(_f32c(d_cls_score)), ptr(_f32c(d_bbox_pred)), B, P, ptr(grad_scale),
+                                          ptr(dh16), ptr(dh32), stream_ptr()), "sb_rpn_head_grad_devscale")
+    else:
+        check(L.sb_rpn_head_grad(ptr(_f32c(d_cls_score)), ptr(_f32c(d_bbox_pred)), B, P, float(grad_scale), ptr(dh16),
+                                 ptr(dh32), stream_ptr()), "sb_rpn_head_grad")
     return dh16, dh32
 
 
 def fpn_grad_combine(dp=None, dt=None, dp6=None, scale=1.0, shape=None, out=None, out16=None, f32=True, f16=True):
     """gradient of one FPN level (NHWC fp32): scale * dp + up^T(dt) + scatter2(scale * dp6), where up^T is the
     transpose of the align_corners bilinear upsample from this level to dt's size and scatter2 the backward of
-    P6 = P5[::2, ::2].  shape = (N, H, W, C) when dp is None.  Returns (fp32, fp16) as requested."""
+    P6 = P5[::2, ::2].  shape = (N, H, W, C) when dp is None.  scale: a host float or an fp32 [1] CUDA tensor read on
+    the device (sb_fpn_grad_combine_devscale).  Returns (fp32, fp16) as requested."""
     L = _l.load()
     N, H, W, C = dp.shape if dp is not None else shape
     dev = next(t.device for t in (dp, dt, dp6) if t is not None)
@@ -584,8 +607,12 @@ def fpn_grad_combine(dp=None, dt=None, dp6=None, scale=1.0, shape=None, out=None
     H6, W6 = (dp6.shape[1], dp6.shape[2]) if dp6 is not None else (0, 0)
     for t in (dp, dt, dp6):
         assert t is None or (t.dtype == torch.float32 and t.shape[0] == N and t.shape[3] == C)
-    check(L.sb_fpn_grad_combine(ptr(dp), ptr(dt), N, H, W, TH, TW, C, ptr(dp6), H6, W6, float(scale), ptr(out),
-                                ptr(out16), stream_ptr()), "sb_fpn_grad_combine")
+    if device_scale(scale):
+        check(L.sb_fpn_grad_combine_devscale(ptr(dp), ptr(dt), N, H, W, TH, TW, C, ptr(dp6), H6, W6, ptr(scale),
+                                             ptr(out), ptr(out16), stream_ptr()), "sb_fpn_grad_combine_devscale")
+    else:
+        check(L.sb_fpn_grad_combine(ptr(dp), ptr(dt), N, H, W, TH, TW, C, ptr(dp6), H6, W6, float(scale), ptr(out),
+                                    ptr(out16), stream_ptr()), "sb_fpn_grad_combine")
     return out, out16
 
 
@@ -599,6 +626,15 @@ def fill_(t, v=0.0):
     L = _l.load()
     assert t.element_size() == 4
     check(L.sb_fill(ptr(t), t.numel(), float(v), stream_ptr()), "sb_fill")
+    return t
+
+
+def fill_reciprocal_(t, v):
+    """t[...] = 1 / v for a contiguous fp32 CUDA tensor t and v an fp32 [1] CUDA tensor, read on the device
+    (sb_fill_reciprocal)"""
+    L = _l.load()
+    assert t.dtype == torch.float32 and device_scale(v)
+    check(L.sb_fill_reciprocal(ptr(t), t.numel(), ptr(v), stream_ptr()), "sb_fill_reciprocal")
     return t
 
 
@@ -729,7 +765,7 @@ def dropout_words_(x, words, p):
 def box_tail_backward(d_cls, d_box, d_dim, fc7, w_cls, w_box, w_dim, grads, mask_scale=1.0, grad_scale=1.0,
                       nonfinite=None):
     """backward of the box tail's three linears: grads = (dw_cls, db_cls, dw_box, db_box, dw_dim, db_dim), written in
-    place -> (dz16, dz32) [R,K], the gradient of RCNN_top.3's pre-activation times grad_scale"""
+    place -> (dz16, dz32) [R,K], the gradient of RCNN_top.3's pre-activation times grad_scale (as in conv_wgrad)"""
     L = _l.load()
     R, K = fc7.shape
     nc = d_cls.shape[1]
@@ -738,17 +774,19 @@ def box_tail_backward(d_cls, d_box, d_dim, fc7, w_cls, w_box, w_dim, grads, mask
         assert g.dtype == torch.float32 and g.is_contiguous() and g.numel() == n
     dz16 = torch.empty(R, K, dtype=torch.float16, device=fc7.device)
     dz32 = torch.empty(R, K, dtype=torch.float32, device=fc7.device)
-    check(L.sb_box_tail_backward(ptr(_f32c(d_cls)), ptr(_f32c(d_box)), ptr(_f32c(d_dim)), ptr(_f32c(fc7)), R, K, nc,
-                                 ptr(w_cls), ptr(w_box), ptr(w_dim), float(mask_scale), float(grad_scale),
-                                 *[ptr(g) for g in grads], ptr(dz16), ptr(dz32), ptr(nonfinite), stream_ptr()),
-          "sb_box_tail_backward")
+    dev = device_scale(grad_scale)
+    fn, name = (L.sb_box_tail_backward_devscale, "sb_box_tail_backward_devscale") if dev else \
+        (L.sb_box_tail_backward, "sb_box_tail_backward")
+    check(fn(ptr(_f32c(d_cls)), ptr(_f32c(d_box)), ptr(_f32c(d_dim)), ptr(_f32c(fc7)), R, K, nc, ptr(w_cls), ptr(w_box),
+             ptr(w_dim), float(mask_scale), ptr(grad_scale) if dev else float(grad_scale), *[ptr(g) for g in grads],
+             ptr(dz16), ptr(dz32), ptr(nonfinite), stream_ptr()), name)
     return dz16, dz32
 
 
 def kpts_tail_backward(up16, w, d_kpts_pred, d_left, d_right, dw, db, db_up, grad_scale=1.0, nonfinite=None):
     """backward of the keypoint tail: up16 [R,G,G,C] the saved deconv output, w [6,C] kpts_class -> dw [6*C], db [6],
     db_up [C] written in place; returns dup16 [R,G/2,G/2,4C], the masked deconv-output gradient times grad_scale in
-    the deconv's four (a, b) phases"""
+    the deconv's four (a, b) phases (grad_scale as in conv_wgrad)"""
     L = _l.load()
     R, G, _, C = up16.shape
     assert up16.dtype == torch.float16 and up16.is_contiguous()
@@ -758,9 +796,12 @@ def kpts_tail_backward(up16, w, d_kpts_pred, d_left, d_right, dw, db, db_up, gra
     dup = torch.empty(R, G // 2, G // 2, 4 * C, dtype=torch.float16, device=up16.device)
     nb = L.sb_kpts_tail_backward_workspace(R, C)
     ws = workspace(nb, up16.device, "kpts_tail_bwd")
-    check(L.sb_kpts_tail_backward(ptr(up16), R, G, C, ptr(w), ptr(_f32c(d_kpts_pred)), ptr(_f32c(d_left)),
-                                  ptr(_f32c(d_right)), float(grad_scale), ptr(dup), ptr(dw), ptr(db), ptr(db_up),
-                                  ptr(nonfinite), ptr(ws), nb, stream_ptr()), "sb_kpts_tail_backward")
+    dev = device_scale(grad_scale)
+    fn, name = (L.sb_kpts_tail_backward_devscale, "sb_kpts_tail_backward_devscale") if dev else \
+        (L.sb_kpts_tail_backward, "sb_kpts_tail_backward")
+    check(fn(ptr(up16), R, G, C, ptr(w), ptr(_f32c(d_kpts_pred)), ptr(_f32c(d_left)), ptr(_f32c(d_right)),
+             ptr(grad_scale) if dev else float(grad_scale), ptr(dup), ptr(dw), ptr(db), ptr(db_up), ptr(nonfinite),
+             ptr(ws), nb, stream_ptr()), name)
     return dup
 
 

@@ -419,6 +419,51 @@ def sgd_step(params, grads, moms, lr, momentum, weight_decay, lr_mult, skip, ski
     return skipped
 
 
+LOSS_SCALE_MIN, LOSS_SCALE_MAX = 2.0 ** -32, 2.0 ** 32      # sb_loss_scale_update's bounds
+
+
+def _fp32_power_of_two(v):
+    """v is a positive power of two that float32 holds exactly"""
+    v = float(v)
+    return v > 0 and np.isfinite(v) and ctypes.c_float(v).value == v and np.frexp(v)[0] == 0.5
+
+
+class DynamicLossScale(object):
+    """torch.cuda.amp.GradScaler's dynamic loss scale for Trainer(grad_scale=DynamicLossScale(...)): the scale starts at
+    init_scale; a step whose backward raised found_inf multiplies it by backoff_factor, growth_interval steps in a row
+    without one multiply it by growth_factor (sb_loss_scale_update).  The scale stays within [2^-32, 2^32]: the fp16
+    chain spans about 2^-24..2^16, so no useful scale lies outside, and power-of-two factors keep the scale and its
+    reciprocal exact.  The constructor raises ValueError for an init_scale that is not a power of two in
+    [LOSS_SCALE_MIN, LOSS_SCALE_MAX], factors that are not powers of two, growth_factor <= 1, backoff_factor >= 1 or
+    growth_interval < 1."""
+
+    def __init__(self, init_scale=2.0 ** 16, growth_factor=2.0, backoff_factor=0.5, growth_interval=2000):
+        if not _fp32_power_of_two(init_scale) or not LOSS_SCALE_MIN <= float(init_scale) <= LOSS_SCALE_MAX:
+            raise ValueError("init_scale must be a power of two in [2^-32, 2^32], got %r" % (init_scale,))
+        if not _fp32_power_of_two(growth_factor) or not float(growth_factor) > 1.0:
+            raise ValueError("growth_factor must be a power of two > 1, got %r" % (growth_factor,))
+        if not _fp32_power_of_two(backoff_factor) or not float(backoff_factor) < 1.0:
+            raise ValueError("backoff_factor must be a power of two < 1, got %r" % (backoff_factor,))
+        if int(growth_interval) != growth_interval or int(growth_interval) < 1:
+            raise ValueError("growth_interval must be an integer >= 1, got %r" % (growth_interval,))
+        self.init_scale, self.growth_factor = float(init_scale), float(growth_factor)
+        self.backoff_factor, self.growth_interval = float(backoff_factor), int(growth_interval)
+
+    def __repr__(self):
+        return "DynamicLossScale(init_scale=%g, growth_factor=%g, backoff_factor=%g, growth_interval=%d)" % (
+            self.init_scale, self.growth_factor, self.backoff_factor, self.growth_interval)
+
+
+def loss_scale_update(found_inf, scale, growth_tracker, growth_factor=2.0, backoff_factor=0.5, growth_interval=2000):
+    """torch._amp_update_scale_ on the device (sb_loss_scale_update), in place: found_inf / growth_tracker int32 [1],
+    scale fp32 [1], all CUDA tensors.  No host synchronisation.  -> scale"""
+    L = _l.load()
+    assert found_inf.dtype == torch.int32 and growth_tracker.dtype == torch.int32 and scale.dtype == torch.float32
+    check(L.sb_loss_scale_update(ptr(found_inf), ptr(scale), ptr(growth_tracker), float(growth_factor),
+                                 float(backoff_factor), int(growth_interval), stream_ptr()), "sb_loss_scale_update")
+    return scale
+
+
 def trainable_names(fixed_blocks=1, n_classes=2):
     """[(name, shape)] of every trainable tensor of the model in the order loss_gradients produces them"""
     from . import engine as E
@@ -459,14 +504,30 @@ class Trainer(object):
     overflow) writes no master, momentum or packed weight and counts itself in `skipped`: GradScaler's skip, the one
     deliberate difference from the reference.  The defaults are the reference's (config.py:22-46,
     trainval_net.py:153-168,226).  `engine` must have been built from `state_dict` (fp16 operands); the constructor
-    uploads the refresh table and synchronises once.  At world > 1 `rank` is dist.get_rank(), otherwise 0."""
+    uploads the refresh table and synchronises once.  At world > 1 `rank` is dist.get_rank(), otherwise 0.
+
+    grad_scale is either a host float, the same constant loss scale in every step, or a DynamicLossScale.  A dynamic
+    scale lives on the device: `loss_scale` (fp32 [1]) and `growth_tracker` (int32 [1]).  Every backward kernel reads
+    the scale there and the unscale vectors are its reciprocal computed on the device, so a captured step follows the
+    scale from replay to replay.  After the SGD step (skipped on found_inf) and the weight refresh, the step runs
+    sb_loss_scale_update on the same found_inf -- at world > 1 the flag already reduced over the ranks, so every rank
+    holds the same scale without another collective: an overflow halves the scale (backoff_factor), growth_interval
+    clean steps in a row double it (growth_factor).  Steps skipped while the scale backs off are counted in
+    `skipped`."""
 
     def __init__(self, engine, state_dict, fixed_blocks=1, lr=1e-3, momentum=0.9, weight_decay=1e-4,
                  double_bias=False, bias_decay=False, clip_norm=10.0, grad_scale=1.0, world=1, dist=None, seed=0):
         self.engine, self.fixed_blocks, self.momentum = engine, int(fixed_blocks), float(momentum)
-        self.clip_norm, self.grad_scale, self.world, self.dist = float(clip_norm), float(grad_scale), int(world), dist
+        self.clip_norm, self.world, self.dist = float(clip_norm), int(world), dist
         self.rank = int(dist.get_rank()) if self.world > 1 and dist is not None else 0
         dev = engine.device
+        self.dynamic = grad_scale if isinstance(grad_scale, DynamicLossScale) else None
+        if self.dynamic is not None:
+            self.loss_scale = torch.full((1,), self.dynamic.init_scale, dtype=torch.float32, device=dev)
+            self.growth_tracker = torch.zeros(1, dtype=torch.int32, device=dev)
+            self.grad_scale = self.loss_scale
+        else:
+            self.grad_scale = float(grad_scale)
         named = trainable_names(fixed_blocks, engine.n_classes)
         self.names = [n for n, _ in named]
         self.masters, self.grads, self.moms = state_buckets([s for _, s in named] + [(6,)], dev, world, dist)
@@ -519,6 +580,10 @@ class Trainer(object):
         clip_gradient(self.grads.grads[:-1], self.clip_norm, out=self.norm)
         self._sgd(self.lr, self.momentum, eng.found_inf, self.skipped)
         eng.refresh_weights(self.params)
+        if self.dynamic is not None:
+            d = self.dynamic
+            loss_scale_update(eng.found_inf, self.loss_scale, self.growth_tracker, d.growth_factor, d.backoff_factor,
+                              d.growth_interval)
         return losses, self.total, self.norm, self.skipped
 
     def step_from_frames(self, inp):
@@ -560,17 +625,23 @@ class Trainer(object):
         "momentum": {name: momentum buffer}} (the buffers of torch.optim.SGD's state, by parameter name, "uncert"
         included), plus what a resumed run needs to continue as if it had not stopped: "epoch" (the next epoch of fit,
         as the reference stores epoch + 1), "step" (the device step counter that keys the random words), "lr" and
-        "sampler_state" (fit's host generator).  A sync point."""
+        "sampler_state" (fit's host generator).  With a DynamicLossScale also "loss_scale" (fp32 [1]) and
+        "growth_tracker" (int32 [1]).  A sync point."""
         mom = {n: v.detach().cpu().clone() for n, v in zip(self.names + ["uncert"], self.moms.grads)}
-        return {"model": self.state_dict(), "uncert": self.uncert.detach().cpu().clone(), "momentum": mom,
-                "epoch": int(self.epoch), "step": int(self.step_count.item()), "lr": self.lr_value,
-                "sampler_state": self.sampler_state}
+        out = {"model": self.state_dict(), "uncert": self.uncert.detach().cpu().clone(), "momentum": mom,
+               "epoch": int(self.epoch), "step": int(self.step_count.item()), "lr": self.lr_value,
+               "sampler_state": self.sampler_state}
+        if self.dynamic is not None:
+            out["loss_scale"] = self.loss_scale.detach().cpu().clone()
+            out["growth_tracker"] = self.growth_tracker.detach().cpu().clone()
+        return out
 
     def load_checkpoint(self, ckpt):
         """Resume from checkpoint(): the masters, uncert, every momentum buffer (which the reference's resume,
         trainval_net.py:170-179, leaves at zero), the step counter, the epoch and the lr, then the engine's packed
-        weights refreshed from the masters.  The frozen tensors are the engine's own: build the engine and the trainer
-        from the state_dict of the run that is resumed.  Host -> device copies: call it outside any capture."""
+        weights refreshed from the masters; a dynamic trainer also restores "loss_scale" and "growth_tracker" when the
+        checkpoint holds them.  The frozen tensors are the engine's own: build the engine and the trainer from the
+        state_dict of the run that is resumed.  Host -> device copies: call it outside any capture."""
         with torch.no_grad():
             for n, v in self.params.items():
                 v.copy_(ckpt["model"][n].to(torch.float32))
@@ -578,6 +649,9 @@ class Trainer(object):
             for n, v in zip(self.names + ["uncert"], self.moms.grads):
                 v.copy_(ckpt["momentum"][n])
             self.step_count.copy_(torch.tensor([int(ckpt["step"])], dtype=torch.int64))
+            if self.dynamic is not None and "loss_scale" in ckpt:
+                self.loss_scale.copy_(ckpt["loss_scale"].reshape(1).to(torch.float32))
+                self.growth_tracker.copy_(ckpt["growth_tracker"].reshape(1).to(torch.int32))
         self.epoch, self.sampler_state = int(ckpt["epoch"]), ckpt.get("sampler_state")
         self.set_lr(ckpt["lr"])
         self.engine.refresh_weights(self.params)
@@ -743,7 +817,8 @@ def fit(trainer, roidb, frames, epochs, start_epoch=1, lr_decay_step=5, lr_decay
     (not scaled with the batch, as in the reference).  Per step rank 0 logs two lines in the reference's format
     (trainval_net.py:240-244) with the losses averaged over the ranks (parallel.average_losses) and [iter k/n] counting
     steps; the numbers are copied to pinned memory behind an event and read one step late, so the steady state has no
-    device-wide synchronise.  With save_dir, rank 0 saves trainer.checkpoint() after every epoch as
+    device-wide synchronise.  A trainer with a DynamicLossScale adds a third line per step, "loss scale: %g, skipped
+    steps: %d", the scale after the step and the trainer's skipped count, read through the same copy.  With save_dir, rank 0 saves trainer.checkpoint() after every epoch as
     stereo_rcnn_{epoch}_{last step}.pth (trainval_net.py:248-254).  To resume, on every rank:
     trainer.load_checkpoint(ckpt), then fit(..., start_epoch=ckpt["epoch"]).
 
@@ -778,6 +853,9 @@ def fit(trainer, roidb, frames, epochs, start_epoch=1, lr_decay_step=5, lr_decay
     val_pipe, val_slots = None, {}
     slots, runners, turn = {}, {}, {}
     stats_host = [torch.zeros(7, dtype=torch.float32).pin_memory() for _ in range(2)]
+    dynamic = trainer.dynamic is not None
+    scale_host = [torch.zeros(1, dtype=torch.float32).pin_memory() for _ in range(2)] if dynamic else None
+    skipped_host = [torch.zeros(1, dtype=torch.int32).pin_memory() for _ in range(2)] if dynamic else None
     stats_ev = [torch.cuda.Event() for _ in range(2)]
     totals = []
 
@@ -803,6 +881,8 @@ def fit(trainer, roidb, frames, epochs, start_epoch=1, lr_decay_step=5, lr_decay
         log("[epoch %2d][iter %4d/%4d] loss: %.4f, lr: %.2e" % (epoch, it, n, v[6], lr))
         log("\t\t\trpn_cls: %.4f, rpn_box_left_right: %.4f, rcnn_cls: %.4f, rcnn_box_left_right %.4f,dim_orien %.4f, "
             "kpts %.4f" % tuple(v[:6]))
+        if dynamic:
+            log("\t\t\tloss scale: %g, skipped steps: %d" % (float(scale_host[k][0]), int(skipped_host[k][0])))
 
     for epoch, lr in lr_schedule(trainer.lr_value, start_epoch, epochs, lr_decay_step, lr_decay_gamma):
         if lr != trainer.lr_value:
@@ -834,6 +914,9 @@ def fit(trainer, roidb, frames, epochs, start_epoch=1, lr_decay_step=5, lr_decay
                 k = it % 2
                 stats_host[k][:6].copy_(out[0], non_blocking=True)
                 stats_host[k][6:].copy_(out[1], non_blocking=True)
+                if dynamic:
+                    scale_host[k].copy_(trainer.loss_scale, non_blocking=True)
+                    skipped_host[k].copy_(trainer.skipped, non_blocking=True)
                 stats_ev[k].record()
             if it > 0:
                 report(1 - k, epoch, it - 1, n, lr)
